@@ -272,10 +272,11 @@ __global__ void __launch_bounds__(kHaloThreads) conv_halo_kernel(const __grid_co
 
 // fp32 channel-last -> channel blocks [c_offset/8, (c_offset + c_cover)/8) of the blocked fp16 pair planes
 // [2][B][C8][H'][W'][8] (the C values of x, then zeros); optional x2 bilinear (align_corners) upsampling on the way.
+// hi_only: the lo plane is left unwritten (1-term operands never read it), which halves the bytes stored.
 // One thread per (pixel, 8-channel block): 32-byte reads, one 16-byte store per plane, consecutive threads = consecutive
 // pixels of one channel block (coalesced 512-byte stores per warp).  c_offset must be a multiple of 8.
 __global__ void split_blocked_kernel(const float* __restrict__ x, __half* __restrict__ planes, int B, int H, int W, int C, int C8,
-                                     int upsample, int c_offset, int c_cover) {
+                                     int upsample, int hi_only, int c_offset, int c_cover) {
   pdl_launch_dependents();
   pdl_wait();
   const int Ho = upsample ? 2 * H : H, Wo = upsample ? 2 * W : W;
@@ -342,7 +343,7 @@ __global__ void split_blocked_kernel(const float* __restrict__ x, __half* __rest
   }
   const size_t o = (((size_t)b * C8 + (c_offset >> 3) + cb) * hw + p_in) * 8;
   *reinterpret_cast<uint4*>(planes + o) = *reinterpret_cast<const uint4*>(hi);
-  *reinterpret_cast<uint4*>(planes + total + o) = *reinterpret_cast<const uint4*>(lo);
+  if (!hi_only) *reinterpret_cast<uint4*>(planes + total + o) = *reinterpret_cast<const uint4*>(lo);
 }
 
 static int make_halo_map(CUtensorMap* map, const void* ptr, int B, int H, int W, int C8, int halo_w, int halo_h, int kc8) {
@@ -445,14 +446,16 @@ extern "C" int dvmvs_conv2d_halo(const dvmvs_conv_halo_desc* d, dvmvs_stream_t s
   return d->ksize == 3 ? launch_halo_kt<64, 3>(p, grid, smem, st) : launch_halo_kt<64, 5>(p, grid, smem, st);
 }
 
-extern "C" int dvmvs_split_blocked(const float* x, void* planes, int B, int H, int W, int C, int C8, int upsample2x, int c_offset,
+extern "C" int dvmvs_split_blocked(const float* x, void* planes, int B, int H, int W, int C, int C8, int flags, int c_offset,
                                    int c_cover, dvmvs_stream_t stream) {
   DVMVS_REQUIRE(x && planes && B > 0 && H > 0 && W > 0 && C > 0 && C8 > 0, "split_blocked: bad argument");
+  DVMVS_REQUIRE((flags & ~(DVMVS_SPLIT_UPSAMPLE2X | DVMVS_SPLIT_HI_ONLY)) == 0, "split_blocked: unknown flags 0x%x", flags);
+  const int upsample2x = (flags & DVMVS_SPLIT_UPSAMPLE2X) ? 1 : 0;
   DVMVS_REQUIRE(c_offset >= 0 && c_cover >= C && c_offset + c_cover <= C8 * 8, "split_blocked: channel window [%d,+%d) outside %d",
                 c_offset, c_cover, C8 * 8);
   DVMVS_REQUIRE(c_offset % 8 == 0, "split_blocked: c_offset must be a multiple of 8 (got %d)", c_offset);
   const size_t total = (size_t)B * H * W * ((c_cover + 7) / 8) * (upsample2x ? 4 : 1);
   launch_k(split_blocked_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, (cudaStream_t)stream, x, (__half*)planes, B, H, W, C,
-           C8, upsample2x, c_offset, c_cover);
+           C8, upsample2x, (flags & DVMVS_SPLIT_HI_ONLY) ? 1 : 0, c_offset, c_cover);
   return check_launch("split_blocked_kernel");
 }

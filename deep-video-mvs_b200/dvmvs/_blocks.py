@@ -114,7 +114,12 @@ class DecoderBlock(NativeModule):
         if fork is not None:
             fork.join()
         srcs = [(x, D), (skip, D)] if depth is None else [(x, D), (skip, D), (depth, U)]   # cat fused (model.py:112-115)
-        return c2.run([(c1.run(srcs), D)])
+        # conv1's output is read only by conv2: on the halo path that is just the blocked planes.  The block's output is read
+        # as fp32 (the depth head, the next block's x2-upsampling loader, the API), so conv2 writes fp32 only.
+        h, w = x.f32.shape[1], x.f32.shape[2]
+        blk_only = c1.path(h, w) == "halo" and c2.path(h, w) == "halo"
+        y = c1.run(srcs, want_f32=not blk_only, want_planes=not blk_only)
+        return c2.run([(y, D)], want_planes=False, want_blk=False)
 
     def forward(self, x, skip, depth):
         return ops.act_to_api(self.run(ops.to_act(x), ops.to_act(skip), None if depth is None else ops.to_act(depth)))
@@ -355,6 +360,8 @@ class CostVolumeDecoder(NativeModule):
         d3 = self.decoder_block3.run(d2, skip1, None, depth_producer=head(1, d2))
         d4 = self.decoder_block4.run(d3, skip0, None, depth_producer=head(2, d3))
         Ho, Wo = 2 * d4.f32.shape[1], 2 * d4.f32.shape[2]
+        # refine.0's output is read only by refine.1 (on the halo path: its blocked planes); refine.1's only by the fp32 depth head
+        r0_out = {"want_f32": False, "want_planes": False} if r0.path(Ho, Wo) == "halo" and r1.path(Ho, Wo) == "halo" else {}
         if r0.pack_sources and r0.path(Ho, Wo) == "halo":
             # refine.0 reads ONE concatenated operand [up(d4), up(sigmoid), image]: the head runs on the side stream while
             # the two sources that exist already are staged; the sigmoid map is staged after the join
@@ -365,12 +372,12 @@ class CostVolumeDecoder(NativeModule):
             buf = ops.split_blocked(meta, only=(0, 2))
             fork.join()
             ops.split_blocked([(d4.f32, True), (s2.f32, True), (image.f32, False)], only=(1,), into=buf)
-            x = r0.run([(d4, U), (s2, U), (image, D)], prestaged=buf)                     # cat order model.py:295
+            x = r0.run([(d4, U), (s2, U), (image, D)], prestaged=buf, **r0_out)           # cat order model.py:295
         else:
             s2 = head(3, d4)()
-            x = r0.run([(d4, U), (s2, U), (image, D)])                                    # cat order model.py:295
+            x = r0.run([(d4, U), (s2, U), (image, D)], **r0_out)                          # cat order model.py:295
         depth16, depth8, depth4, depth2 = depths[0], depths[1], depths[2], depths[3]
-        x = r1.run([(x, D)])
+        x = r1.run([(x, D)], want_planes=False, want_blk=False)
         _, depth1 = heads[4].run([(x, D)], aux=aux)
         return [t.squeeze(3) for t in (depth1, depth2, depth4, depth8, depth16)]
 

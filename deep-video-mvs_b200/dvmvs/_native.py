@@ -12,6 +12,7 @@ _lib = None
 
 ACT_NONE, ACT_RELU, ACT_SIGMOID = 0, 1, 2
 SRC_DIRECT, SRC_UPSAMPLE2X = 0, 1
+SPLIT_UPSAMPLE2X, SPLIT_HI_ONLY = 1, 2
 RES_NONE, RES_SAME, RES_NEAREST_UP = 0, 1, 2
 SWEEP_DOT, SWEEP_SAD = 0, 1
 LOSS_L1, LOSS_L1_INV, LOSS_L1_REL, LOSS_HUBER = 0, 1, 2, 3

@@ -544,7 +544,8 @@ def split_blocked(sources, only=None, into=None):
     8-channel block boundary: narrow sources (the 1-channel depth, the RGB image) are padded to 8 with zero channels --
     PackedConvHalo(pad_sources_to_8=True) lays the weights out the same way.
     only / into: stage just the listed source indices into an existing operand tensor (sources not staged yet may be
-    given as (shape tuple, upsample)) -- lets independent producers fill one concatenated operand at different times."""
+    given as (shape tuple, upsample)) -- lets independent producers fill one concatenated operand at different times.
+    While no kernel reads lo planes (1-term operands everywhere) only the hi plane is written."""
     shp = lambda t: tuple(t) if isinstance(t, (tuple, list)) else tuple(t.shape)
     shapes = [(shp(t)[1] * (2 if up else 1), shp(t)[2] * (2 if up else 1)) for t, up in sources]
     B, (Ho, Wo) = shp(sources[0][0])[0], shapes[0]
@@ -555,12 +556,14 @@ def split_blocked(sources, only=None, into=None):
         dev = next(t.device for t, _ in sources if isinstance(t, torch.Tensor))
         into = torch.empty((2, B, C8, Ho, Wo, 8), dtype=torch.float16, device=dev)
     planes = into
+    hi_only = 0 if lo_planes_needed() else N.SPLIT_HI_ONLY
     off = 0
     for i, (t, up) in enumerate(sources):
         C = shp(t)[3]
         cover = (C + 7) // 8 * 8
         if only is None or i in only:
-            N.check(N.lib().dvmvs_split_blocked(t.data_ptr(), planes.data_ptr(), B, t.shape[1], t.shape[2], C, C8, 1 if up else 0, off, cover,
+            flags = (N.SPLIT_UPSAMPLE2X if up else 0) | hi_only
+            N.check(N.lib().dvmvs_split_blocked(t.data_ptr(), planes.data_ptr(), B, t.shape[1], t.shape[2], C, C8, flags, off, cover,
                                                 _stream()), "split_blocked")
         off += cover
     return planes
@@ -948,14 +951,24 @@ class ConvLayer:
             return r
         return None
 
-    def run(self, sources, residual=None, residual_mode=N.RES_NONE, aux=None, want_f32=True, want_planes=True, prestaged=None):
+    def run(self, sources, residual=None, residual_mode=N.RES_NONE, aux=None, want_f32=True, want_planes=True, want_blk=True,
+            prestaged=None):
         """sources: list of (Act, mode).  Returns Act (or (Act, aux tensor)).  want_* only prune outputs of the
-        tensor-core path (the fp32 path always produces fp32).  prestaged: the concatenated blocked operand of a
-        pack_sources layer on the halo path, already filled by the caller (split_blocked(..., only=, into=))."""
+        tensor-core path (the fp32 path always produces fp32): want_f32 the fp32 tensor, want_planes the fp16 pair
+        planes (what tensor-core consumers read), want_blk (halo path only) the blocked planes (what halo consumers read
+        for SRC_DIRECT).  Callers prune an output only when they know every consumer of the result reads another one.
+        prestaged: the concatenated blocked operand of a pack_sources layer on the halo path, already filled by the
+        caller (split_blocked(..., only=, into=))."""
         pc = self.pc
         a0, m0 = sources[0]
-        hin = (a0.f32 if a0.f32 is not None else a0.planes[0]).shape[1] * (2 if m0 == N.SRC_UPSAMPLE2X else 1)
-        win = (a0.f32 if a0.f32 is not None else a0.planes[0]).shape[2] * (2 if m0 == N.SRC_UPSAMPLE2X else 1)
+        if a0.f32 is not None:
+            hin, win = a0.f32.shape[1], a0.f32.shape[2]
+        elif a0.planes is not None:
+            hin, win = a0.planes.shape[2], a0.planes.shape[3]
+        else:
+            hin, win = a0.blk.shape[3], a0.blk.shape[4]
+        if m0 == N.SRC_UPSAMPLE2X:
+            hin, win = 2 * hin, 2 * win
         if self.uses_halo(hin, win, residual_mode, aux):
             if self._phalo is None:
                 self._phalo = PackedConvHalo(pc, self.src_channels, pc.weight.device, concat_padded=self.pack_sources)
@@ -968,7 +981,7 @@ class ConvLayer:
                         (a.blk_up if (mode == N.SRC_UPSAMPLE2X and a.blk_up is not None) else split_blocked([(a.f32, mode == N.SRC_UPSAMPLE2X)]))
                         for a, mode in sources]
             f32, oblk, onhwc = conv2d_halo(blks, self._phalo, residual=residual.f32 if residual is not None else None,
-                                           terms=_TC_TERMS, want_f32=True, want_blk=True, want_nhwc=want_planes)
+                                           terms=_TC_TERMS, want_f32=want_f32, want_blk=want_blk, want_nhwc=want_planes)
             return Act(f32, onhwc, oblk)
         if self.uses_tc():
             if self._ptc is None:

@@ -36,6 +36,7 @@ enum {
 
 enum { DVMVS_ACT_NONE = 0, DVMVS_ACT_RELU = 1, DVMVS_ACT_SIGMOID = 2 };
 enum { DVMVS_SRC_DIRECT = 0, DVMVS_SRC_UPSAMPLE2X = 1 };     /* conv input source modes */
+enum { DVMVS_SPLIT_UPSAMPLE2X = 1, DVMVS_SPLIT_HI_ONLY = 2 };   /* dvmvs_split_blocked flags */
 enum { DVMVS_RES_NONE = 0, DVMVS_RES_SAME = 1, DVMVS_RES_NEAREST_UP = 2 };
 enum { DVMVS_SWEEP_DOT = 0, DVMVS_SWEEP_SAD = 1 };
 enum { DVMVS_LOSS_L1 = 0, DVMVS_LOSS_L1_INV = 1, DVMVS_LOSS_L1_REL = 2, DVMVS_LOSS_HUBER = 3 };   /* losses.py:33-40 loss_type */
@@ -206,8 +207,10 @@ typedef struct {
 int dvmvs_conv2d_halo(const dvmvs_conv_halo_desc* desc_host, dvmvs_stream_t stream);
 
 /* fp32 channel-last [B][H][W][C] -> channels [c_offset, c_offset + c_cover) of the BLOCKED fp16 pair planes
- * [2][B][C8][H'][W'][8] (x, then zeros), optional x2 bilinear (align_corners) upsampling (H' = 2H). */
-int dvmvs_split_blocked(const float* x, void* planes, int B, int H, int W, int C, int C8, int upsample2x, int c_offset,
+ * [2][B][C8][H'][W'][8] (x, then zeros).  flags: DVMVS_SPLIT_UPSAMPLE2X applies x2 bilinear (align_corners) upsampling
+ * (H' = 2H; the value 1 keeps its earlier meaning), DVMVS_SPLIT_HI_ONLY leaves the lo plane unwritten (for operands only
+ * 1-term products read). */
+int dvmvs_split_blocked(const float* x, void* planes, int B, int H, int W, int C, int C8, int flags, int c_offset,
                         int c_cover, dvmvs_stream_t stream);
 
 /* fp32 channel-last [B][H][W][C] -> channels [c_offset, c_offset + c_cover) of fp16 (hi, lo) planes

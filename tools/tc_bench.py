@@ -1,9 +1,16 @@
 """Steady-state timing (CUDA events, warm caches, back-to-back launches) of individual convolution layers on both
-backends, for the layer shapes that dominate the keyframe.  Usage: python tools/tc_bench.py [terms]"""
+backends, for the layer shapes that dominate the keyframe.  Usage: python tools/tc_bench.py [terms]
+
+    python tools/tc_bench.py halo [terms]
+
+times every halo convolution (dvmvs_conv2d_halo) of bench.py's default engine at the shape and with the outputs the engine
+runs it: the engine is built and primed, each conv2d_halo call it makes is recorded with its operands, and each distinct
+call is then replayed alone.  Prints us and achieved TFLOP/s (2 x MACs / time) per layer, then a JSON record."""
 import os
 import sys
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, REPO)
 sys.path.insert(0, os.path.join(REPO, "deep-video-mvs_b200"))
 import torch
 
@@ -43,7 +50,89 @@ def timeit(fn, iters=30):
     return e0.elapsed_time(e1) / iters * 1e3
 
 
+def layer_names(mods):
+    """id(ConvLayer) -> 'tag.module[index]' for every packed layer of the modules"""
+    names = {}
+
+    def walk(obj, path):
+        if isinstance(obj, ops.ConvLayer):
+            names[id(obj)] = path
+        elif isinstance(obj, (list, tuple)):
+            for i, o in enumerate(obj):
+                walk(o, "%s[%d]" % (path, i))
+
+    for tag, m in mods.items():
+        for name, sub in m.named_modules():
+            walk(getattr(sub, "_packed", None), tag + ("." + name if name else ""))
+    return names
+
+
+def halo_layers(terms):
+    import json
+
+    import bench
+    from dvmvs import pipeline
+    from dvmvs.fusionnet.model import CostVolumeDecoder, CostVolumeEncoder, FeatureExtractor, FeatureShrinker, LSTMFusion
+    ops.set_conv_backend("tc", terms=1, stride2=True)
+    dev = torch.device(DEV, 0)
+    H, W, D, M = bench.H, bench.W, bench.D, bench.M
+    mods = {"fe": FeatureExtractor(), "fpn": FeatureShrinker(), "cve": CostVolumeEncoder(), "lstm": LSTMFusion(), "cvd": CostVolumeDecoder()}
+    for m in mods.values():
+        shapes = {k: tuple(v.shape) for k, v in m.state_dict().items()}
+        m.load_state_dict({k: torch.from_numpy(v) for k, v in synth.make_state_dict(shapes, seed=7).items()}, strict=True)
+        m.to(dev).eval()
+    clip = [synth.make_clip(0, 1, H, W, M)]
+    ref, rpose, meas, mpose, K = bench.stack_frame(clip, 0)
+    frame = (torch.from_numpy(ref).to(dev), torch.from_numpy(rpose).to(dev), [torch.from_numpy(x).to(dev) for x in meas],
+             [torch.from_numpy(p).to(dev) for p in mpose], torch.from_numpy(K).to(dev))
+    calls, layer_of = {}, {}
+    real_halo, real_run = ops.conv2d_halo, ops.ConvLayer.run
+    current = []
+
+    def run(self, *a, **k):
+        current.append(self)
+        try:
+            return real_run(self, *a, **k)
+        finally:
+            current.pop()
+
+    def record(sources_blk, ph, residual=None, **kw):
+        key = (id(ph), tuple(sources_blk[0].shape))
+        if key not in calls:
+            calls[key] = (list(sources_blk), ph, residual, kw)
+            layer_of[key] = current[-1] if current else None
+        return real_halo(sources_blk, ph, residual=residual, **kw)
+
+    ops.conv2d_halo, ops.ConvLayer.run = record, run
+    try:
+        eng = pipeline.LookaheadFusionnet(mods, batch=1, height=H, width=W, n_measurement_frames=M, n_depth_levels=D, lookahead=4)
+        with torch.no_grad():
+            eng.prime(*frame)
+        eng.synchronize()
+    finally:
+        ops.conv2d_halo, ops.ConvLayer.run = real_halo, real_run
+    names = layer_names(mods)
+    rows = []
+    with torch.no_grad():
+        for key, (blks, ph, residual, kw) in calls.items():
+            kw = dict(kw, terms=terms)
+            B, Hh, Ww = blks[0].shape[1], blks[0].shape[3], blks[0].shape[4]
+            t = timeit(lambda: real_halo(blks, ph, residual=residual, **kw), iters=100)
+            macs = B * Hh * Ww * ph.cout * ph.cin * ph.ksize * ph.ksize
+            lay = layer_of[key]
+            rows.append({"layer": names.get(id(lay), "?"), "B": B, "H": Hh, "W": Ww, "cin": ph.cin, "cout": ph.cout, "k": ph.ksize,
+                         "kc": ph.kc, "block_n": ph.block_n, "outputs": [o for o in ("f32", "blk", "nhwc") if kw.get("want_" + o, o != "blk")],
+                         "us": t, "tflops": 2.0 * macs / (t * 1e-6) / 1e12})
+    rows.sort(key=lambda r: -r["us"])
+    for r in rows:
+        print("%-28s B=%-2d %3dx%-3d %3d->%-3d k%d kc%d N%d %-14s %8.1f us %6.1f TFLOP/s" % (
+            r["layer"], r["B"], r["H"], r["W"], r["cin"], r["cout"], r["k"], r["kc"], r["block_n"], "+".join(r["outputs"]), r["us"], r["tflops"]))
+    print(json.dumps({"device": torch.cuda.get_device_name(0), "terms": terms, "total_us": sum(r["us"] for r in rows), "layers": rows}))
+
+
 def main():
+    if len(sys.argv) > 1 and sys.argv[1] == "halo":
+        return halo_layers(int(sys.argv[2]) if len(sys.argv) > 2 else 1)
     terms = int(sys.argv[1]) if len(sys.argv) > 1 else 3
     for name, B, H, W, chans, Cout, k, stride in LAYERS:
         cin = sum(chans)
