@@ -28,6 +28,7 @@
 #include <math.h>
 #include <stdlib.h>
 
+#include "color_fold.cuh"
 #include "common.cuh"
 
 namespace dvmvs {
@@ -52,13 +53,6 @@ struct TsdfParams {
 
 __device__ __forceinline__ float np_minimum(float a, float b) { return (a != a) ? a : ((b != b) ? b : (a < b ? a : b)); }
 __device__ __forceinline__ double np_minimum(double a, double b) { return (a != a) ? a : ((b != b) ? b : (a < b ? a : b)); }
-
-__device__ __forceinline__ void unfold(float c, float& b, float& g, float& r) {
-  b = floorf(__fdiv_rn(c, 65536.f));
-  const float rest = __fsub_rn(c, __fmul_rn(b, 65536.f));
-  g = floorf(__fdiv_rn(rest, 256.f));
-  r = __fsub_rn(rest, __fmul_rn(g, 256.f));
-}
 
 constexpr int kTsdfRun = 8;      // consecutive z voxels per thread: one frustum test covers the whole run
 

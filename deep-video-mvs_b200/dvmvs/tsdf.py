@@ -6,8 +6,13 @@ a GPU the constructor raises.
 
 Same constructor / integrate / get_volume signatures and argument meaning as the reference (:34, :220, :325).  `integrate`
 accepts numpy arrays (as the reference's caller passes, :500-560) or CUDA tensors (depth maps straight from the network:
-no host round trip).  Mesh extraction (marching cubes, :329-358) is scikit-image's job in the reference too and is delegated to
-it when installed."""
+no host round trip).
+
+Mesh extraction (`get_mesh` / `get_point_cloud`, :329-358), scikit-image's marching cubes in the reference, runs on the device
+too: dvmvs_mesh_count / dvmvs_mesh_extract (csrc/mesh.cu).  Sign-only face resolution makes the mesh watertight wherever it
+does not reach the volume border, and its order deterministic (vertices by grid edge, faces by cube); the contract is stated in
+csrc/mesh.cu and tools/gen_mc_tables.py.  `get_mesh_tensors` leaves the mesh on the device; `get_mesh` copies only the mesh
+(never the volume) to the host."""
 import ctypes
 
 import numpy as np
@@ -111,25 +116,33 @@ class TSDFVolume(object):
         """Total number of voxel updates so far (synchronises)."""
         return int(self._updated.item())
 
-    def _colors_at(self, color_vol, verts_ind):
-        rgb_vals = color_vol[verts_ind[:, 0], verts_ind[:, 1], verts_ind[:, 2]]
-        b = np.floor(rgb_vals / self._color_const)
-        g = np.floor((rgb_vals - b * self._color_const) / 256)
-        r = rgb_vals - b * self._color_const - g * 256
-        return np.floor(np.asarray([r, g, b])).T.astype(np.uint8)
+    def get_mesh_tensors(self):
+        """Marching cubes at level 0 on the device (:344-358): (verts (V,3) float32 world coordinates, faces (F,3) int32,
+        norms (V,3) float32, colors (V,3) uint8 RGB) as CUDA tensors, enqueued on torch's current stream.  Synchronises
+        once: the host reads the vertex and face counts between the count and the extract launches to size the outputs."""
+        dims = [int(d) for d in self._vol_dim]
+        with torch.cuda.device(self.device):
+            nbytes = ctypes.c_longlong(0)
+            N.check(N.lib().dvmvs_mesh_scratch_bytes(dims[0], dims[1], dims[2], ctypes.byref(nbytes)), "mesh_scratch_bytes")
+            scratch = torch.empty(max(int(nbytes.value), 8), dtype=torch.uint8, device=self.device)
+            stream = _stream()
+            N.check(N.lib().dvmvs_mesh_count(self._tsdf_vol.data_ptr(), dims[0], dims[1], dims[2], scratch.data_ptr(),
+                                             scratch.numel(), stream), "mesh_count")
+            n_verts, n_faces = (int(v) for v in scratch[:8].view(torch.int32).cpu())        # the one device -> host read
+            verts = torch.empty((n_verts, 3), dtype=torch.float32, device=self.device)
+            norms = torch.empty((n_verts, 3), dtype=torch.float32, device=self.device)
+            colors = torch.empty((n_verts, 3), dtype=torch.uint8, device=self.device)
+            faces = torch.empty((n_faces, 3), dtype=torch.int32, device=self.device)
+            keys = torch.empty(max(n_verts, 1), dtype=torch.int32, device=self.device)
+            N.check(N.lib().dvmvs_mesh_extract(
+                self._tsdf_vol.data_ptr(), self._color_vol.data_ptr(), dims[0], dims[1], dims[2], self._origin_c,
+                self._voxel_size, scratch.data_ptr(), scratch.numel(), n_verts, n_faces, keys.data_ptr(), verts.data_ptr(),
+                faces.data_ptr(), norms.data_ptr(), colors.data_ptr(), stream), "mesh_extract")
+        return verts, faces, norms, colors
 
     def get_mesh(self):
-        """:344-358 -- marching cubes is scikit-image's in the reference as well."""
-        try:
-            from skimage import measure
-        except ImportError:
-            raise RuntimeError("TSDFVolume.get_mesh needs scikit-image (marching cubes), as the reference does")
-        tsdf_vol, color_vol = self.get_volume()
-        mc = getattr(measure, "marching_cubes_lewiner", None) or measure.marching_cubes
-        verts, faces, norms, _ = mc(tsdf_vol, level=0)
-        verts_ind = np.round(verts).astype(int)
-        verts = verts * self._voxel_size + self._vol_origin
-        return verts, faces, norms, self._colors_at(color_vol, verts_ind)
+        """(verts, faces, norms, colors) as numpy arrays, like the reference's :344-358: get_mesh_tensors copied to the host."""
+        return tuple(t.cpu().numpy() for t in self.get_mesh_tensors())
 
     def get_point_cloud(self):
         """:329-342."""

@@ -330,6 +330,30 @@ int dvmvs_tsdf_integrate(float* tsdf_vol, float* weight_vol, float* color_vol, i
                          const double* world_to_cam16, double obs_weight, unsigned long long* updated_count,
                          dvmvs_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------
+ * Marching cubes on the TSDF volume: replaces the reference's scikit-image call in TSDFVolume.get_mesh
+ * (run-tsdf-reconstruction.py:344-358, and get_point_cloud :329-342 through it).  Contract (inside = tsdf < 0, sign-only
+ * face resolution, vertex / normal / colour arithmetic, output order) in csrc/mesh.cu and tools/gen_mc_tables.py.
+ * Two calls with one device-to-host read between them, which the caller makes to size the outputs:
+ *   dvmvs_mesh_scratch_bytes  HOST query: bytes of scratch for a volume (proportional to the voxel count / 65536)
+ *   dvmvs_mesh_count          classifies every cube and grid edge and scans the per-CTA counts; the first two ints of
+ *                             scratch are then (n_verts, n_faces)
+ *   dvmvs_mesh_extract        with the same volume and scratch: verts [n_verts][3] fp32 world coordinates, norms
+ *                             [n_verts][3] fp32 unit normals (toward increasing tsdf), colors [n_verts][3] uint8 RGB, faces
+ *                             [n_faces][3] int32 vertex ids (counter-clockwise seen from the normal side); vertex_keys
+ *                             [n_verts] int32 is scratch for the face ids.
+ *   tsdf_vol, color_vol : DEVICE fp32 [dim_x][dim_y][dim_z] (C order), colour folded b*65536 + g*256 + r
+ *   vol_origin_host     : HOST, 3 floats (:52)            voxel_size : the float32 voxel size (:351)
+ * A volume with a dimension < 2 (0 included) has an empty mesh.  DVMVS_EINVAL when dim_x * dim_y * dim_z * 5 exceeds INT32_MAX (the
+ * int32 counts, keys and face ids). */
+int dvmvs_mesh_scratch_bytes(int dim_x, int dim_y, int dim_z, long long* bytes_host);
+int dvmvs_mesh_count(const float* tsdf_vol, int dim_x, int dim_y, int dim_z, void* scratch, long long scratch_bytes,
+                     dvmvs_stream_t stream);
+int dvmvs_mesh_extract(const float* tsdf_vol, const float* color_vol, int dim_x, int dim_y, int dim_z,
+                       const float* vol_origin_host, float voxel_size, const void* scratch, long long scratch_bytes, int n_verts,
+                       int n_faces, int* vertex_keys, float* verts, int* faces, float* norms, unsigned char* colors,
+                       dvmvs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
