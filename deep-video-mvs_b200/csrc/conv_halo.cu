@@ -212,23 +212,26 @@ __global__ void __launch_bounds__(kHaloThreads) conv_halo_kernel(const __grid_co
       }
     }
     asm volatile("bar.sync 1, 128;" ::: "memory");
-    const int row = warp * 32 + lane;
-    const float* srow = stg + row * kPitch;
-    const int ty = row >> 3, tx = row & 7;
-    const int oy = oy0 + ty, ox = ox0 + tx;
-    const bool valid = (oy < p.Hout) && (ox < p.Wout);
     if (threadIdx.x == 0) HALO_MARK(5);
-    const size_t pix = ((size_t)b * p.Hout + oy) * p.Wout + ox;
     const size_t hw = (size_t)p.Hout * p.Wout;
     const size_t plane_elems = (size_t)p.B * p.c8_out * hw * 8;
     const size_t nhwc_plane = (size_t)p.B * hw * p.Cout;
+    // One thread per (pixel, 8-channel chunk).  A channel-last output (fp32 or fp16 planes) is written chunks fastest:
+    // consecutive threads store consecutive pieces of one pixel row of the tile, so a warp's stores are contiguous runs.
+    // The blocked output alone is written pixels fastest: 8 consecutive pixels of one channel block are 128 contiguous bytes.
+    constexpr int kChunks = BLOCK_N / 8;
+    const bool chunks_fastest = p.out_f32 || p.out_nhwc;
 #pragma unroll 1
-    for (int c0 = 0; c0 < BLOCK_N; c0 += 8) {
-      float v[8];
-      *reinterpret_cast<float4*>(v) = *reinterpret_cast<const float4*>(srow + c0);
-      *reinterpret_cast<float4*>(v + 4) = *reinterpret_cast<const float4*>(srow + c0 + 4);
+    for (int item = threadIdx.x; item < 128 * kChunks; item += 128) {
+      const int row = chunks_fastest ? item / kChunks : item % 128;
+      const int c0 = 8 * (chunks_fastest ? item % kChunks : item / 128);
+      const int oy = oy0 + (row >> 3), ox = ox0 + (row & 7);
       const int cbase = n0 + c0;
-      if (!valid || cbase >= p.Cout) continue;
+      if (oy >= p.Hout || ox >= p.Wout || cbase >= p.Cout) continue;
+      const size_t pix = ((size_t)b * p.Hout + oy) * p.Wout + ox;
+      float v[8];
+      *reinterpret_cast<float4*>(v) = *reinterpret_cast<const float4*>(stg + row * kPitch + c0);
+      *reinterpret_cast<float4*>(v + 4) = *reinterpret_cast<const float4*>(stg + row * kPitch + c0 + 4);
       if (p.bias) {
         const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + cbase)), b1 = __ldg(reinterpret_cast<const float4*>(p.bias + cbase + 4));
         v[0] += b0.x; v[1] += b0.y; v[2] += b0.z; v[3] += b0.w; v[4] += b1.x; v[5] += b1.y; v[6] += b1.z; v[7] += b1.w;

@@ -258,32 +258,28 @@ __global__ void __launch_bounds__(kTcThreads) conv_tc_kernel(const __grid_consta
       }
     }
     asm volatile("bar.sync 1, 128;" ::: "memory");
-    const int row = warp * 32 + lane;
-    const float* srow = stg + row * kPitch;
-    const int ty = row / p.tile_w, tx = row - ty * p.tile_w;
-    const int oy = oy0 + ty, ox = ox0 + tx;
-    const bool valid = (oy < p.Hout) && (ox < p.Wout);
-    const size_t pix = ((size_t)b * p.Hout + oy) * p.Wout + ox;
     const size_t plane_stride = (size_t)p.B * p.Hout * p.Wout * p.Cout;
     const bool split = p.ksplit > 1;
-    float* wsp_row = split ? p.workspace + (size_t)blockIdx.z * plane_stride + pix * p.Cout : nullptr;
-    const float* res_row = nullptr;
-    if (p.residual_mode == DVMVS_RES_SAME) {
-      res_row = p.residual + pix * p.Cout;
-    } else if (p.residual_mode == DVMVS_RES_NEAREST_UP) {
-      const int ry = (int)(((long long)oy * p.Hr) / p.Hout), rx = (int)(((long long)ox * p.Wr) / p.Wout);
-      res_row = p.residual + (((size_t)b * p.Hr + ry) * p.Wr + rx) * p.Cout;
-    }
     const bool vec8 = (p.Cout & 7) == 0;
     // compact, rolled epilogue (8 accumulator columns per iteration): keeps the kernel's code footprint small -- these
-    // kernels are short, an unrolled 32-column epilogue costs more in instruction fetch than it saves in issue slots
+    // kernels are short, an unrolled 32-column epilogue costs more in instruction fetch than it saves in issue slots.
+    // One thread per (pixel, 8-channel chunk), chunks fastest: consecutive threads store consecutive 32-byte (fp32) /
+    // 16-byte (fp16) pieces of one channel-last pixel row, i.e. a warp writes whole contiguous runs of the output instead
+    // of one 16-byte piece per pixel (a stride of Cout elements between lanes).  The staging reads are conflict-free for
+    // BLOCK_N = 32 (the pitch of BLOCK_N + 4 floats puts the next pixel's chunks four banks further), two-way for wider tiles.
+    constexpr int kChunks = BLOCK_N / 8;
 #pragma unroll 1
-    for (int c0 = 0; c0 < BLOCK_N; c0 += 8) {
-      float v[8];
-      *reinterpret_cast<float4*>(v) = *reinterpret_cast<const float4*>(srow + c0);
-      *reinterpret_cast<float4*>(v + 4) = *reinterpret_cast<const float4*>(srow + c0 + 4);
+    for (int item = threadIdx.x; item < kTileM * kChunks; item += 128) {
+      const int row = item / kChunks, c0 = 8 * (item - row * kChunks);
+      const int ty = row / p.tile_w, tx = row - ty * p.tile_w;
+      const int oy = oy0 + ty, ox = ox0 + tx;
       const int cbase = n0 + c0;
-      if (!valid || cbase >= p.Cout) continue;
+      if (oy >= p.Hout || ox >= p.Wout || cbase >= p.Cout) continue;
+      const size_t pix = ((size_t)b * p.Hout + oy) * p.Wout + ox;
+      float v[8];
+      *reinterpret_cast<float4*>(v) = *reinterpret_cast<const float4*>(stg + row * kPitch + c0);
+      *reinterpret_cast<float4*>(v + 4) = *reinterpret_cast<const float4*>(stg + row * kPitch + c0 + 4);
+      float* wsp_row = split ? p.workspace + (size_t)blockIdx.z * plane_stride + pix * p.Cout : nullptr;
       if (vec8) {
         if (split) {
           // partial sums of this tap range; conv_tc_finish_kernel reduces the splits in fixed order
@@ -293,6 +289,13 @@ __global__ void __launch_bounds__(kTcThreads) conv_tc_kernel(const __grid_consta
         }
         tc_emit8(p, v, b, oy, ox, cbase);
       } else {        // generic tail (Cout not a multiple of 8): scalar, rolled
+        const float* res_row = nullptr;
+        if (p.residual_mode == DVMVS_RES_SAME) {
+          res_row = p.residual + pix * p.Cout;
+        } else if (p.residual_mode == DVMVS_RES_NEAREST_UP) {
+          const int ry = (int)(((long long)oy * p.Hr) / p.Hout), rx = (int)(((long long)ox * p.Wr) / p.Wout);
+          res_row = p.residual + (((size_t)b * p.Hr + ry) * p.Wr + rx) * p.Cout;
+        }
 #pragma unroll 1
         for (int e = 0; e < 8; ++e) {
           const int c = cbase + e;

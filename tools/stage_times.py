@@ -4,6 +4,9 @@ back, and reports microseconds and kernel launches per stage beside the steady-s
 The last stage carries the loop dependence (ConvLSTM state + previous depth): the period cannot drop below its latency.
 
     python tools/stage_times.py [--clips 1] [--stages 5] [--out profiles/r02_stage_times.json]
+
+--lookahead N times LookaheadFusionnet instead: its period, each batched stage's graph alone (per group of N keyframes) and the
+recurrent stage's graph alone (per keyframe), whose share of the period says whether the loop-carried chain bounds it.
 """
 import argparse
 import json
@@ -83,8 +86,33 @@ def main():
             la.synchronize()
             torch.cuda.synchronize()
             period = e0.elapsed_time(e1) * 1e3 / (3 * (n_frames - 8))
+
+            def alone(graph, stream, reps):
+                with torch.cuda.stream(stream):
+                    for _ in range(10):
+                        graph.replay()
+                    q0, q1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    q0.record(stream)
+                    for _ in range(reps):
+                        graph.replay()
+                    q1.record(stream)
+                    stream.synchronize()
+                return q0.elapsed_time(q1) * 1e3 / reps
+
+            # each stage's graph replayed alone: the batched stages once per group of `lookahead` keyframes, the recurrent
+            # stage once per keyframe (its replays advance the static recurrent state, restored afterwards as _graph_of does)
+            grp = la.groups[0]
+            batched = [alone(grp["graph"][i], la.streams[i], max(a.reps, 50)) for i in range(4)]
+            saved = [t.clone() for t in la._static_state]
+            ks = next(k for k in la.kslots if True in k["graph"])
+            rec_us = alone(ks["graph"][True], la.streams[4], max(a.reps, 200))
+            for dst, src in zip(la._static_state, saved):
+                dst.copy_(src)
+            torch.cuda.synchronize()
         print(json.dumps({"engine": "LookaheadFusionnet", "lookahead": a.lookahead, "groups": a.groups, "clips": a.clips,
                           "period_us_per_keyframe_batch": period, "keyframes_per_s": a.clips * 1e6 / period, "host_enqueue_us_per_submit": host_us,
+                          "recurrent_stage_us_alone": rec_us, "recurrent_stage_share_of_period": rec_us / period,
+                          "batched_stages_us_alone_per_group": batched, "batched_stages_us_alone_per_keyframe": sum(batched) / a.lookahead,
                           "launches_per_keyframe": la.kernels_per_keyframe, "kernels": list(la._kernels),
                           "rel_l1_depth_vs_pipelined_engine_first_14_keyframes_max": max(errs), "finite": bool(torch.isfinite(out).all())}))
         return

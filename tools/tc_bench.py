@@ -5,7 +5,12 @@ backends, for the layer shapes that dominate the keyframe.  Usage: python tools/
 
 times every halo convolution (dvmvs_conv2d_halo) of bench.py's default engine at the shape and with the outputs the engine
 runs it: the engine is built and primed, each conv2d_halo call it makes is recorded with its operands, and each distinct
-call is then replayed alone.  Prints us and achieved TFLOP/s (2 x MACs / time) per layer, then a JSON record."""
+call is then replayed alone.  Prints us and achieved TFLOP/s (2 x MACs / time) per layer, then a JSON record.
+
+    python tools/tc_bench.py tc
+
+does the same for every dvmvs_conv2d_tc call of the engine.  Both modes mark the calls the engine issues on its recurrent
+(loop-carried) stage with "rec"."""
 import os
 import sys
 
@@ -50,6 +55,31 @@ def timeit(fn, iters=30):
     return e0.elapsed_time(e1) / iters * 1e3
 
 
+def graph_timeit(fn, calls=20, replays=20):
+    """us per call of `fn` with `calls` back-to-back calls captured in one CUDA graph: the device time the engine's graphs see.
+    Timing eager calls instead measures the host (Python, descriptor, allocation: ~20-30 us per call), not these kernels."""
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        for _ in range(3):
+            fn()
+    s.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g, stream=s):
+        for _ in range(calls):
+            fn()
+    for _ in range(3):
+        g.replay()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(replays):
+        g.replay()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / (calls * replays) * 1e3
+
+
 def layer_names(mods):
     """id(ConvLayer) -> 'tag.module[index]' for every packed layer of the modules"""
     names = {}
@@ -67,9 +97,9 @@ def layer_names(mods):
     return names
 
 
-def halo_layers(terms):
-    import json
-
+def engine_calls(kind):
+    """Builds and primes bench.py's default engine with every `kind` ('halo' or 'tc') convolution call recorded: returns
+    (mods, {key: (args, kwargs, ConvLayer or None, on the recurrent stage?)})."""
     import bench
     from dvmvs import pipeline
     from dvmvs.fusionnet.model import CostVolumeDecoder, CostVolumeEncoder, FeatureExtractor, FeatureShrinker, LSTMFusion
@@ -85,54 +115,99 @@ def halo_layers(terms):
     ref, rpose, meas, mpose, K = bench.stack_frame(clip, 0)
     frame = (torch.from_numpy(ref).to(dev), torch.from_numpy(rpose).to(dev), [torch.from_numpy(x).to(dev) for x in meas],
              [torch.from_numpy(p).to(dev) for p in mpose], torch.from_numpy(K).to(dev))
-    calls, layer_of = {}, {}
-    real_halo, real_run = ops.conv2d_halo, ops.ConvLayer.run
-    current = []
+    name = "conv2d_halo" if kind == "halo" else "conv2d_tc"
+    real_conv, real_run, real_deferred = getattr(ops, name), ops.ConvLayer.run, ops.ConvLayer.run_deferred
+    calls, current, rec_stream = {}, [], []
 
-    def run(self, *a, **k):
-        current.append(self)
-        try:
-            return real_run(self, *a, **k)
-        finally:
-            current.pop()
+    def within(real):
+        def fn(self, *a, **k):
+            current.append(self)
+            try:
+                return real(self, *a, **k)
+            finally:
+                current.pop()
+        return fn
 
-    def record(sources_blk, ph, residual=None, **kw):
-        key = (id(ph), tuple(sources_blk[0].shape))
+    def record(sources, packed, *a, **kw):
+        key = (id(packed), tuple(sources[0].shape), bool(kw.get("defer_finish")))
         if key not in calls:
-            calls[key] = (list(sources_blk), ph, residual, kw)
-            layer_of[key] = current[-1] if current else None
-        return real_halo(sources_blk, ph, residual=residual, **kw)
+            on_rec = bool(rec_stream) and torch.cuda.current_stream(dev) == rec_stream[0]
+            calls[key] = ((list(sources), packed) + a, kw, current[-1] if current else None, on_rec)
+        return real_conv(sources, packed, *a, **kw)
 
-    ops.conv2d_halo, ops.ConvLayer.run = record, run
+    setattr(ops, name, record)
+    ops.ConvLayer.run, ops.ConvLayer.run_deferred = within(real_run), within(real_deferred)
     try:
         eng = pipeline.LookaheadFusionnet(mods, batch=1, height=H, width=W, n_measurement_frames=M, n_depth_levels=D, lookahead=4)
+        rec_stream.append(eng.streams[4])
         with torch.no_grad():
             eng.prime(*frame)
         eng.synchronize()
     finally:
-        ops.conv2d_halo, ops.ConvLayer.run = real_halo, real_run
+        setattr(ops, name, real_conv)
+        ops.ConvLayer.run, ops.ConvLayer.run_deferred = real_run, real_deferred
+    return mods, calls
+
+
+def halo_layers(terms):
+    import json
+    mods, calls = engine_calls("halo")
     names = layer_names(mods)
     rows = []
     with torch.no_grad():
-        for key, (blks, ph, residual, kw) in calls.items():
+        for key, (args, kw, lay, on_rec) in calls.items():
+            blks, ph = args[0], args[1]
             kw = dict(kw, terms=terms)
             B, Hh, Ww = blks[0].shape[1], blks[0].shape[3], blks[0].shape[4]
-            t = timeit(lambda: real_halo(blks, ph, residual=residual, **kw), iters=100)
+            t = graph_timeit(lambda: ops.conv2d_halo(*args, **kw))
+            t_eager = timeit(lambda: ops.conv2d_halo(*args, **kw), iters=100)
             macs = B * Hh * Ww * ph.cout * ph.cin * ph.ksize * ph.ksize
-            lay = layer_of[key]
-            rows.append({"layer": names.get(id(lay), "?"), "B": B, "H": Hh, "W": Ww, "cin": ph.cin, "cout": ph.cout, "k": ph.ksize,
-                         "kc": ph.kc, "block_n": ph.block_n, "outputs": [o for o in ("f32", "blk", "nhwc") if kw.get("want_" + o, o != "blk")],
-                         "us": t, "tflops": 2.0 * macs / (t * 1e-6) / 1e12})
+            rows.append({"layer": names.get(id(lay), "?"), "recurrent": on_rec, "B": B, "H": Hh, "W": Ww, "cin": ph.cin, "cout": ph.cout,
+                         "k": ph.ksize, "kc": ph.kc, "block_n": ph.block_n,
+                         "outputs": [o for o in ("f32", "blk", "nhwc") if kw.get("want_" + o, o != "blk")],
+                         "us": t, "us_eager": t_eager, "tflops": 2.0 * macs / (t * 1e-6) / 1e12})
     rows.sort(key=lambda r: -r["us"])
     for r in rows:
-        print("%-28s B=%-2d %3dx%-3d %3d->%-3d k%d kc%d N%d %-14s %8.1f us %6.1f TFLOP/s" % (
-            r["layer"], r["B"], r["H"], r["W"], r["cin"], r["cout"], r["k"], r["kc"], r["block_n"], "+".join(r["outputs"]), r["us"], r["tflops"]))
-    print(json.dumps({"device": torch.cuda.get_device_name(0), "terms": terms, "total_us": sum(r["us"] for r in rows), "layers": rows}))
+        print("%-28s %s B=%-2d %3dx%-3d %3d->%-3d k%d kc%d N%d %-14s %8.1f us %6.1f TFLOP/s (eager %5.1f us)" % (
+            r["layer"], "rec" if r["recurrent"] else "   ", r["B"], r["H"], r["W"], r["cin"], r["cout"], r["k"], r["kc"], r["block_n"],
+            "+".join(r["outputs"]), r["us"], r["tflops"], r["us_eager"]))
+    print(json.dumps({"device": torch.cuda.get_device_name(0), "timing": "graph_timeit", "terms": terms, "total_us": sum(r["us"] for r in rows),
+                      "recurrent_us": sum(r["us"] for r in rows if r["recurrent"]), "layers": rows}))
+
+
+def tc_layers():
+    """every conv2d_tc call of the engine (stride 1 and 2, split-K or not, deferred finishing pass or not) replayed alone"""
+    import json
+    mods, calls = engine_calls("tc")
+    names = layer_names(mods)
+    rows = []
+    with torch.no_grad():
+        for key, (args, kw, lay, on_rec) in calls.items():
+            planes, ptc = args[0], args[1]
+            B, Hin, Win = planes[0].shape[1], planes[0].shape[2], planes[0].shape[3]
+            pad = (ptc.ksize - 1) // 2
+            Ho, Wo = (Hin + 2 * pad - ptc.ksize) // ptc.stride + 1, (Win + 2 * pad - ptc.ksize) // ptc.stride + 1
+            t = graph_timeit(lambda: ops.conv2d_tc(*args, **kw))
+            t_eager = timeit(lambda: ops.conv2d_tc(*args, **kw), iters=100)
+            macs = B * Ho * Wo * ptc.cout * ptc.cin * ptc.ksize * ptc.ksize
+            rows.append({"layer": names.get(id(lay), "?"), "recurrent": on_rec, "B": B, "Hin": Hin, "Win": Win, "Hout": Ho, "Wout": Wo,
+                         "cin": ptc.cin, "sources": [int(p.shape[4]) for p in planes], "cout": ptc.cout, "k": ptc.ksize,
+                         "stride": ptc.stride, "deferred_finish": bool(kw.get("defer_finish")), "us": t, "us_eager": t_eager,
+                         "tflops": 2.0 * macs / (t * 1e-6) / 1e12})
+    rows.sort(key=lambda r: -r["us"])
+    for r in rows:
+        print("%-28s %s B=%-2d %3dx%-3d s%d %4d->%-4d k%d%s %8.1f us %6.1f TFLOP/s (eager %5.1f us)" % (
+            r["layer"], "rec" if r["recurrent"] else "   ", r["B"], r["Hout"], r["Wout"], r["stride"], r["cin"], r["cout"], r["k"],
+            " deferred" if r["deferred_finish"] else "", r["us"], r["tflops"], r["us_eager"]))
+    print(json.dumps({"device": torch.cuda.get_device_name(0), "timing": "graph_timeit", "total_us": sum(r["us"] for r in rows),
+                      "recurrent_us": sum(r["us"] for r in rows if r["recurrent"]), "layers": rows}))
 
 
 def main():
     if len(sys.argv) > 1 and sys.argv[1] == "halo":
         return halo_layers(int(sys.argv[2]) if len(sys.argv) > 2 else 1)
+    if len(sys.argv) > 1 and sys.argv[1] == "tc":
+        return tc_layers()
     terms = int(sys.argv[1]) if len(sys.argv) > 1 else 3
     for name, B, H, W, chans, Cout, k, stride in LAYERS:
         cin = sum(chans)
