@@ -199,7 +199,11 @@ class FeatureExtractor(NativeModule):
             outs = [x]
         for blocks in {"all": levels, "head": levels[:2], "tail": levels[2:]}[part]:
             for expand, dw, project, residual in blocks:
-                y = depthwise(expand.run([(x, D)], want_planes=False), dw, project)
+                if expand.uses_tc():
+                    # expansion + depthwise in one launch: the expanded tensor never leaves shared memory
+                    y = ops.Act(None, ops.expand_dwconv(x, expand, dw))
+                else:
+                    y = depthwise(expand.run([(x, D)], want_planes=False), dw, project)
                 x = project.run([(y, D)], residual=x if residual else None,
                                 residual_mode=N.RES_SAME if residual else N.RES_NONE)
             outs.append(x)

@@ -20,7 +20,7 @@ LOSS_L1, LOSS_L1_INV, LOSS_L1_REL, LOSS_HUBER = 0, 1, 2, 3
 # every symbol include/dvmvs_b200.h declares (tests check that the library exports all of them)
 EXPORTED_SYMBOLS = [
     "dvmvs_abi_version", "dvmvs_set_programmatic_launch", "dvmvs_last_error_string", "dvmvs_kernel_launch_count", "dvmvs_plane_sweep_fused",
-    "dvmvs_hidden_warp", "dvmvs_depth_reproject", "dvmvs_conv2d", "dvmvs_conv2d_tc", "dvmvs_conv2d_halo", "dvmvs_split_blocked", "dvmvs_split_planes", "dvmvs_stem_conv", "dvmvs_dwconv2d", "dvmvs_lstm_gates",
+    "dvmvs_hidden_warp", "dvmvs_depth_reproject", "dvmvs_conv2d", "dvmvs_conv2d_tc", "dvmvs_conv2d_halo", "dvmvs_split_blocked", "dvmvs_split_planes", "dvmvs_stem_conv", "dvmvs_dwconv2d", "dvmvs_expand_dwconv", "dvmvs_lstm_gates",
     "dvmvs_upsample2x", "dvmvs_nchw_to_nhwc", "dvmvs_nhwc_to_nchw", "dvmvs_preprocess_rgb", "dvmvs_tsdf_integrate",
     "dvmvs_plane_sweep_backward", "dvmvs_hidden_warp_backward", "dvmvs_lstm_gates_backward", "dvmvs_depth_loss_forward",
     "dvmvs_depth_loss_backward", "dvmvs_plane_sweep_fused_h16", "dvmvs_plane_sweep_tc", "dvmvs_lstm_gates_parts", "dvmvs_conv2d_tc_ksplit", "dvmvs_plane_sweep_tc_set_timeline",
@@ -122,6 +122,7 @@ def lib():
         L.dvmvs_split_planes.argtypes = [p, p, i, i, i, i, i, i, i, i, p]
         L.dvmvs_stem_conv.argtypes = [p, p, p, p, i, i, i, p]
         L.dvmvs_dwconv2d.argtypes = [p, p, p, p, p, i, i, i, i, i, i, i, p]
+        L.dvmvs_expand_dwconv.argtypes = [p, i, i, i, i, p, p, i, i, p, i, p, p, i, i, i, i, i, i, p, p]
         L.dvmvs_lstm_gates.argtypes = [p, p, p, p, i, i, i, i, p]
         L.dvmvs_lstm_gates_parts.argtypes = [p, i, ctypes.c_longlong, p, p, p, p, i, i, i, i, p]
         L.dvmvs_conv2d_tc_ksplit.argtypes = [ctypes.POINTER(ConvTcDesc)]

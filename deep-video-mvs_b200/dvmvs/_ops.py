@@ -536,6 +536,35 @@ def conv2d_tc(sources, ptc, residual=None, residual_mode=N.RES_NONE, aux=None, w
     return out_f32, out_planes
 
 
+@on_tensor_device
+def expand_dwconv(act, expand_layer, dw, terms=None):
+    """MnasNet block front half in one launch: the 1x1 expansion `expand_layer` (a ConvLayer on the tensor-core path) of the Act
+    `act`, then the depthwise convolution `dw` (PackedDepthwise).  Returns the fp16 (hi, lo) planes (2,B,Hout,Wout,mid) that the
+    block's projection reads -- equal to conv2d_tc(..., want_f32=True) followed by dwconv2d(..., want_planes=True).  The lo plane
+    is written only for terms=3 (the projection runs the same terms); terms=None uses the current family's terms."""
+    terms = _TC_TERMS if terms is None else int(terms)
+    pc = expand_layer.pc
+    if pc.ksize != 1 or pc.stride != 1 or not expand_layer.tc_eligible() or dw.channels != pc.cout:
+        raise ValueError("expand_dwconv: needs a tensor-core 1x1 expansion to %d channels, got k=%d stride=%d cout=%d"
+                         % (dw.channels, pc.ksize, pc.stride, pc.cout))
+    if expand_layer._ptc is None:
+        expand_layer._ptc = PackedConvTC(pc, expand_layer.src_channels, pc.weight.device)
+    ptc = expand_layer._ptc
+    x = act.get_planes()
+    _, B, H, W, Cs = x.shape
+    if Cs != ptc.src_stored[0]:
+        raise ValueError("expand_dwconv: input has %d channels, weights packed for %d" % (Cs, ptc.src_stored[0]))
+    pad = dw.ksize // 2
+    Hout = (H + 2 * pad - dw.ksize) // dw.stride + 1
+    Wout = (W + 2 * pad - dw.ksize) // dw.stride + 1
+    planes = torch.empty((2, B, Hout, Wout, dw.channels), dtype=torch.float16, device=x.device)
+    N.check(N.lib().dvmvs_expand_dwconv(x.data_ptr(), B, H, W, Cs, ptc.w_hi.data_ptr(), ptc.w_lo.data_ptr(), ptc.rows, ptc.ktot,
+                                        ptc.bias.data_ptr(), ptc.act, dw.weight.data_ptr(), dw.bias.data_ptr(), dw.ksize, dw.stride,
+                                        dw.act, dw.channels, terms, 1 if terms == 3 else 0, planes.data_ptr(), _stream()),
+            "expand_dwconv")
+    return planes
+
+
 # ================================================================================================ halo (blocked-layout) path
 @on_tensor_device
 def split_blocked(sources, only=None, into=None):

@@ -232,6 +232,17 @@ int dvmvs_stem_conv(const float* image_nchw, const float* weight, const float* b
 int dvmvs_dwconv2d(const float* x, const float* weight, const float* bias, float* y, void* y_planes, int B, int H, int W,
                    int C, int ksize, int stride, int act, dvmvs_stream_t stream);
 
+/* MnasNet inverted-residual front half in one launch (csrc/expand_dw.cu): the 1x1 expansion Cs -> mid on the tensor cores
+ * (+ bias, expand_act) followed by the depthwise k x k convolution (+ bias, dw_act); the expanded tensor stays in shared
+ * memory.  Results are bit-identical to dvmvs_conv2d_tc (1x1, out_f32) followed by dvmvs_dwconv2d (y_planes).
+ *   x_planes      fp16 (hi, lo) planes [2][B][H][W][Cs] of the block input, Cs a multiple of 8 (plane 1 unused when terms == 1)
+ *   w_hi / w_lo   the expansion's dvmvs_conv2d_tc weights [w_rows][ktot] (ksize 1, one source of Cs channels)
+ *   dw_weight     [k][k][mid], dw_bias [mid]; ksize 3 or 5, stride 1 or 2, mid a multiple of 8
+ *   y_planes      fp16 (hi, lo) [2][B][Hout][Wout][mid]; plane 1 is written only when write_lo != 0. */
+int dvmvs_expand_dwconv(const void* x_planes, int B, int H, int W, int Cs, const void* w_hi, const void* w_lo, int w_rows, int ktot,
+                        const float* expand_bias, int expand_act, const float* dw_weight, const float* dw_bias, int ksize, int stride,
+                        int dw_act, int mid, int terms, int write_lo, void* y_planes, dvmvs_stream_t stream);
+
 /* ConvLSTM gate epilogue: replaces dvmvs/convlstm.py:45-59.  gates [B][h][w][4*C] in the order i,f,o,g;
  * c_in [B][h][w][C]; writes h_out, c_out [B][h][w][C].  LayerNorm over (h,w) per (b,channel), biased
  * variance, eps 1e-5, no affine; CELU alpha = 1. */

@@ -10,7 +10,12 @@ call is then replayed alone.  Prints us and achieved TFLOP/s (2 x MACs / time) p
     python tools/tc_bench.py tc
 
 does the same for every dvmvs_conv2d_tc call of the engine.  Both modes mark the calls the engine issues on its recurrent
-(loop-carried) stage with "rec"."""
+(loop-carried) stage with "rec".
+
+    python tools/tc_bench.py expand [terms]
+
+times the front half (1x1 expansion + depthwise) of every MnasNet trunk block at batch 12 and 3: the two-launch composition
+beside the fused dvmvs_expand_dwconv, with algorithmic HBM bytes, TB/s and TFLOP/s."""
 import os
 import sys
 
@@ -203,11 +208,71 @@ def tc_layers():
                       "recurrent_us": sum(r["us"] for r in rows if r["recurrent"]), "layers": rows}))
 
 
+def expand_layers(terms):
+    """every MnasNet trunk block's front half (1x1 expansion + depthwise) at the engine's shapes -- batch 12 (the lookahead
+    engine's trunk graphs: 4 keyframes x 3 images) and batch 3 -- as the two launches conv2d_tc (fp32 out) + dwconv2d (planes
+    out) and as the fused expand_dwconv; algorithmic HBM bytes (operands in, outputs out, weights ignored) and FLOP/s
+    (expansion at the input resolution + depthwise taps) over graph-timed us"""
+    import json
+    from dvmvs._blocks import FeatureExtractor
+    fe = FeatureExtractor()
+    shapes, side = [], 128
+    for layer in (fe.layer2, fe.layer3, fe.layer4, fe.layer5):
+        for stack in layer:
+            for blk in stack:
+                L = blk.layers
+                shapes.append((L[0].in_channels, L[0].out_channels, L[3].kernel_size[0], blk.stride, side))
+                side //= blk.stride
+    rows = []
+    planes_in = 2 if terms == 3 else 1
+    with torch.no_grad():
+        for B in (12, 3):
+            for shape in sorted(set(shapes), key=shapes.index):
+                cin, mid, k, s, H = shape
+                w = torch.from_numpy(synth.tensor("tb/we", (mid, cin, 1, 1), seed=2, scale=(2.0 / cin) ** 0.5)).to(DEV)
+                bias = torch.from_numpy(synth.tensor("tb/be", (mid,), seed=3, scale=0.1)).to(DEV)
+                expand = ops.ConvLayer(ops.PackedConv(w, bias, None, act=N.ACT_RELU))
+                bn = torch.nn.BatchNorm2d(mid).to(DEV).eval()
+                dw = ops.PackedDepthwise(torch.from_numpy(synth.tensor("tb/wd", (mid, 1, k, k), seed=4, scale=0.3)).to(DEV), bn, stride=s)
+                x = ops.Act(torch.from_numpy(synth.tensor("tb/x", (B, H, H, cin), seed=1)).to(DEV))
+                planes = x.get_planes()
+                ptc = ops.PackedConvTC(expand.pc, [cin], DEV)
+                Ho = (H + 2 * (k // 2) - k) // s + 1
+
+                def two_launch():
+                    f32, _ = ops.conv2d_tc([planes], ptc, terms=terms, want_f32=True, want_planes=False)
+                    ops.dwconv2d(f32, dw, want_f32=False, want_planes=True)
+
+                t_old = graph_timeit(two_launch)
+                t_new = graph_timeit(lambda: ops.expand_dwconv(x, expand, dw, terms))
+                x_bytes, e_bytes, y_bytes = planes_in * B * H * H * cin * 2, B * H * H * mid * 4, B * Ho * Ho * mid * 2
+                old_bytes = x_bytes + 2 * e_bytes + 2 * y_bytes                  # dwconv_kernel writes both planes
+                new_bytes = x_bytes + planes_in * y_bytes
+                flops = 2.0 * B * H * H * cin * mid * terms + 2.0 * B * Ho * Ho * mid * k * k
+                rows.append({"B": B, "cin": cin, "mid": mid, "k": k, "stride": s, "Hin": H, "Hout": Ho, "blocks": shapes.count(shape),
+                             "us_two_launch": t_old, "us_fused": t_new, "mb_two_launch": old_bytes / 1e6, "mb_fused": new_bytes / 1e6,
+                             "tbs_two_launch": old_bytes / (t_old * 1e-6) / 1e12, "tbs_fused": new_bytes / (t_new * 1e-6) / 1e12,
+                             "tflops_two_launch": flops / (t_old * 1e-6) / 1e12, "tflops_fused": flops / (t_new * 1e-6) / 1e12})
+    for r in rows:
+        print("B=%-2d %3d->%-4d k%d s%d %3d^2->%3d^2 x%d | two launches %7.1f us %6.1f MB %5.2f TB/s %5.1f TFLOP/s | fused %7.1f us %6.1f MB "
+              "%5.2f TB/s %5.1f TFLOP/s | x%.2f" % (
+                  r["B"], r["cin"], r["mid"], r["k"], r["stride"], r["Hin"], r["Hout"], r["blocks"], r["us_two_launch"], r["mb_two_launch"],
+                  r["tbs_two_launch"], r["tflops_two_launch"], r["us_fused"], r["mb_fused"], r["tbs_fused"], r["tflops_fused"],
+                  r["us_two_launch"] / r["us_fused"]))
+    for B in (12, 3):
+        sel = [r for r in rows if r["B"] == B]
+        print("B=%d, all 16 blocks: two launches %.1f us, fused %.1f us" % (
+            B, sum(r["us_two_launch"] * r["blocks"] for r in sel), sum(r["us_fused"] * r["blocks"] for r in sel)))
+    print(json.dumps({"device": torch.cuda.get_device_name(0), "timing": "graph_timeit", "terms": terms, "blocks": rows}))
+
+
 def main():
     if len(sys.argv) > 1 and sys.argv[1] == "halo":
         return halo_layers(int(sys.argv[2]) if len(sys.argv) > 2 else 1)
     if len(sys.argv) > 1 and sys.argv[1] == "tc":
         return tc_layers()
+    if len(sys.argv) > 1 and sys.argv[1] == "expand":
+        return expand_layers(int(sys.argv[2]) if len(sys.argv) > 2 else 1)
     terms = int(sys.argv[1]) if len(sys.argv) > 1 else 3
     for name, B, H, W, chans, Cout, k, stride in LAYERS:
         cin = sum(chans)
