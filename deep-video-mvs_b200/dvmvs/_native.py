@@ -24,7 +24,7 @@ EXPORTED_SYMBOLS = [
     "dvmvs_upsample2x", "dvmvs_nchw_to_nhwc", "dvmvs_nhwc_to_nchw", "dvmvs_preprocess_rgb", "dvmvs_tsdf_integrate",
     "dvmvs_plane_sweep_backward", "dvmvs_hidden_warp_backward", "dvmvs_lstm_gates_backward", "dvmvs_depth_loss_forward",
     "dvmvs_depth_loss_backward", "dvmvs_plane_sweep_fused_h16", "dvmvs_plane_sweep_tc", "dvmvs_lstm_gates_parts", "dvmvs_conv2d_tc_ksplit", "dvmvs_plane_sweep_tc_set_timeline",
-    "dvmvs_mesh_scratch_bytes", "dvmvs_mesh_count", "dvmvs_mesh_extract",
+    "dvmvs_mesh_scratch_bytes", "dvmvs_mesh_count", "dvmvs_mesh_extract", "dvmvs_tsdf_raycast",
 ]
 
 
@@ -137,6 +137,7 @@ def lib():
         L.dvmvs_mesh_scratch_bytes.argtypes = [i, i, i, ctypes.POINTER(ll)]
         L.dvmvs_mesh_count.argtypes = [p, i, i, i, p, ll, p]
         L.dvmvs_mesh_extract.argtypes = [p, p, i, i, i, ctypes.POINTER(ctypes.c_float), f, p, ll, i, i, p, p, p, p, p, p]
+        L.dvmvs_tsdf_raycast.argtypes = [p, p, i, i, i, ctypes.POINTER(ctypes.c_float), d, d, p, i, i, i, p, p, p, p]
         L.dvmvs_plane_sweep_backward.argtypes = [p, p, p, p, p, p, p, p, i, i, i, i, i, i, f, f, i, p]
         L.dvmvs_hidden_warp_backward.argtypes = [p, p, p, p, p, p, i, i, i, i, f, p]
         L.dvmvs_lstm_gates_backward.argtypes = [p, p, p, p, p, p, i, i, i, i, p]

@@ -12,7 +12,11 @@ Mesh extraction (`get_mesh` / `get_point_cloud`, :329-358), scikit-image's march
 too: dvmvs_mesh_count / dvmvs_mesh_extract (csrc/mesh.cu).  Sign-only face resolution makes the mesh watertight wherever it
 does not reach the volume border, and its order deterministic (vertices by grid edge, faces by cube); the contract is stated in
 csrc/mesh.cu and tools/gen_mc_tables.py.  `get_mesh_tensors` leaves the mesh on the device; `get_mesh` copies only the mesh
-(never the volume) to the host."""
+(never the volume) to the host.
+
+Rendering (`render` / `render_tensors`), which the reference lacks: depth, normal and colour maps of the fused model at any
+camera poses, ray-cast on the device by dvmvs_tsdf_raycast (csrc/raycast.cu, contract stated there), e.g. to score the fused
+depth against ground truth with dvmvs.errors.compute_errors or as model-to-frame depth for tracking."""
 import ctypes
 
 import numpy as np
@@ -148,6 +152,62 @@ class TSDFVolume(object):
         """:329-342."""
         verts, _, _, colors = self.get_mesh()
         return np.hstack([verts, colors])
+
+    # ---- rendering (no reference counterpart) ---------------------------------------------------------------------------
+    def render_tensors(self, cam_intr, cam_poses, height, width):
+        """Ray-cast the fused volume at one or more camera poses (dvmvs_tsdf_raycast, csrc/raycast.cu; one launch for all
+        views, enqueued on torch's current stream).  cam_intr (3,3) in pixels of the rendered (height, width) image, fx and fy
+        finite and > 0; cam_poses (4,4) or (V,4,4) camera-to-world like integrate's cam_pose, a numpy array or a tensor (CUDA
+        tensors on the volume's device are read there, no host round trip).  Returns CUDA tensors depth (V,H,W) float32
+        camera depth of the first + -> - crossing of the tsdf (0 = no hit), normals (V,H,W,3) float32 world-frame unit normals
+        toward increasing tsdf and colors (V,H,W,3) uint8 RGB (both 0 where there is no hit); a single (4,4) pose gives them
+        without the V axis.  The raw tsdf is rendered: unobserved voxels are not masked (as in get_mesh)."""
+        intr = np.asarray(cam_intr.detach().cpu() if isinstance(cam_intr, torch.Tensor) else cam_intr)
+        if intr.shape != (3, 3):
+            raise RuntimeError("TSDFVolume.render: cam_intr must be (3,3), got %s" % (intr.shape,))
+        intr4 = intr.astype(np.float32)[[0, 1, 0, 1], [0, 1, 2, 2]]                  # fx fy cx cy
+        if not (np.all(np.isfinite(intr4)) and intr4[0] > 0 and intr4[1] > 0):
+            raise RuntimeError("TSDFVolume.render: focal lengths must be finite and > 0 and the principal point finite, got "
+                               "fx %r fy %r cx %r cy %r" % tuple(float(v) for v in intr4))
+        height, width = int(height), int(width)
+        if height <= 0 or width <= 0:
+            raise RuntimeError("TSDFVolume.render: bad image size %d x %d" % (height, width))
+        poses = cam_poses
+        if isinstance(poses, torch.Tensor) and poses.device.type == "cpu":
+            poses = poses.detach().numpy()
+        if not isinstance(poses, torch.Tensor):
+            poses = np.asarray(poses)
+        shape = tuple(poses.shape)
+        single = shape == (4, 4)
+        if not (single or (len(shape) == 3 and shape[0] > 0 and shape[1:] == (4, 4))):
+            raise RuntimeError("TSDFVolume.render: cam_poses must be (4,4) or (V,4,4), got %s" % (shape,))
+        n = 1 if single else shape[0]
+        with torch.cuda.device(self.device):
+            if isinstance(poses, torch.Tensor):
+                if poses.device != self.device:
+                    raise RuntimeError("TSDFVolume.render: cam_poses lives on %s, the volume on %s" % (poses.device, self.device))
+                p = poses.detach().reshape(n, 4, 4)
+                intr_dev = self._upload(torch.from_numpy(intr4.copy()), "intr")             # pinned: no stream synchronisation
+                views = torch.cat([intr_dev.expand(n, 4), p[:, :3, :3].reshape(n, 9).to(torch.float32), p[:, :3, 3].to(torch.float32)],
+                                  dim=1).contiguous()
+            else:
+                p = poses.reshape(n, 4, 4).astype(np.float32)
+                packed = np.concatenate([np.broadcast_to(intr4, (n, 4)), p[:, :3, :3].reshape(n, 9), p[:, :3, 3]], axis=1)
+                views = self._upload(torch.from_numpy(np.ascontiguousarray(packed, dtype=np.float32)), "views")
+            depth = torch.empty((n, height, width), dtype=torch.float32, device=self.device)
+            normals = torch.empty((n, height, width, 3), dtype=torch.float32, device=self.device)
+            colors = torch.empty((n, height, width, 3), dtype=torch.uint8, device=self.device)
+            N.check(N.lib().dvmvs_tsdf_raycast(
+                self._tsdf_vol.data_ptr(), self._color_vol.data_ptr(), int(self._vol_dim[0]), int(self._vol_dim[1]),
+                int(self._vol_dim[2]), self._origin_c, self._voxel_size, self._trunc_margin, views.data_ptr(), n, height, width,
+                depth.data_ptr(), normals.data_ptr(), colors.data_ptr(), _stream()), "tsdf_raycast")
+        if single:
+            return depth[0], normals[0], colors[0]
+        return depth, normals, colors
+
+    def render(self, cam_intr, cam_poses, height, width):
+        """render_tensors copied to the host: (depth, normals, colors) numpy arrays."""
+        return tuple(t.cpu().numpy() for t in self.render_tensors(cam_intr, cam_poses, height, width))
 
 
 class TSDFFusion(object):

@@ -365,6 +365,26 @@ int dvmvs_mesh_extract(const float* tsdf_vol, const float* color_vol, int dim_x,
                        int n_faces, int* vertex_keys, float* verts, int* faces, float* norms, unsigned char* colors,
                        dvmvs_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------
+ * Ray casting of the TSDF volume (TSDFVolume.render): what a camera sees of the fused model.  New: the reference has no
+ * counterpart (its volume's only way out is the mesh).  One launch for all views, one thread per pixel ray; the ray through
+ * integer pixel (u, v) is marched on a lattice of half-voxel steps clipped to the volume box, with an empty-space skip over
+ * fully truncated cells, and stops at the first + -> - crossing of the trilinear tsdf.  Contract (operation order, skip rule)
+ * in csrc/raycast.cu.
+ *   tsdf_vol, color_vol : DEVICE fp32 [dim_x][dim_y][dim_z] (C order), colour folded b*65536 + g*256 + r; the weight volume is
+ *                         not read (the raw tsdf is rendered, as get_mesh meshes it)
+ *   vol_origin3         : HOST, 3 floats            voxel_size, trunc_margin : doubles (trunc_margin sets the skip length)
+ *   views               : DEVICE fp32 [n_views][16]: fx fy cx cy (pixels of the rendered image), R (3x3 row-major,
+ *                         camera -> world, as integrate's cam_pose), t
+ *   depth               : DEVICE fp32 [n_views][im_h][im_w], camera depth of the hit, 0 = no hit
+ *   normals             : DEVICE fp32 [n_views][im_h][im_w][3], world-frame unit normal toward increasing tsdf, 0 = no hit
+ *   colors              : DEVICE uint8 [n_views][im_h][im_w][3] RGB, 0 = no hit
+ * A volume with a dimension < 2 gives no hits.  DVMVS_EINVAL on null pointers, non-positive extents or view counts, and
+ * n_views * im_h * im_w beyond INT32_MAX.  Allocates nothing, does not synchronise. */
+int dvmvs_tsdf_raycast(const float* tsdf_vol, const float* color_vol, int dim_x, int dim_y, int dim_z, const float* vol_origin3,
+                       double voxel_size, double trunc_margin, const float* views, int n_views, int im_h, int im_w, float* depth,
+                       float* normals, unsigned char* colors, dvmvs_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
