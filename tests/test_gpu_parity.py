@@ -88,6 +88,14 @@ def test_plane_sweep_tensor_core_form_vs_reference_golden(synth, cases, golden_o
         got = out.permute(0, 3, 1, 2).cpu().numpy()
         err = rel_err(got, golden_ops["plane_sweep/" + name])
         assert np.isfinite(got).all() and err <= tol, "plane_sweep_tc/%s terms=%d: %.3e" % (name, terms, err)
+        # the fp32 gather kernel fed the SAME rounded features (hi planes, or hi + lo): at terms=3 only the summation order differs
+        # (2e-5); at terms=1 the kernel also keeps its correlations in fp16 before blending them (<= one fp16 ulp, 2^-10)
+        rounded = (lambda p: p[0].float()) if terms == 1 else (lambda p: p[0].float() + p[1].float())
+        same = ops.plane_sweep(rounded(ref), [rounded(m) for m in meas], _cuda(inp["pose1"]), [_cuda(p) for p in inp["pose2s"]],
+                               _cuda(inp["K"]), c["min_depth"], c["max_depth"], c["D"], dot_product=True)
+        err = rel_err(out.cpu().numpy(), same.cpu().numpy())
+        assert err <= (2e-5 if terms == 3 else 2.0 ** -10), "plane_sweep_tc/%s terms=%d vs the gather kernel on the same operands: %.3e" % (
+            name, terms, err)
 
 
 @pytest.mark.parametrize("qcap", [512, 64])

@@ -27,6 +27,7 @@ import torch
 import synth_data as synth
 from dvmvs import _native as N
 from dvmvs import _ops as ops
+from tools.engine_record import engine_calls, layer_names
 
 DEV = "cuda"
 LAYERS = [
@@ -85,78 +86,9 @@ def graph_timeit(fn, calls=20, replays=20):
     return e0.elapsed_time(e1) / (calls * replays) * 1e3
 
 
-def layer_names(mods):
-    """id(ConvLayer) -> 'tag.module[index]' for every packed layer of the modules"""
-    names = {}
-
-    def walk(obj, path):
-        if isinstance(obj, ops.ConvLayer):
-            names[id(obj)] = path
-        elif isinstance(obj, (list, tuple)):
-            for i, o in enumerate(obj):
-                walk(o, "%s[%d]" % (path, i))
-
-    for tag, m in mods.items():
-        for name, sub in m.named_modules():
-            walk(getattr(sub, "_packed", None), tag + ("." + name if name else ""))
-    return names
-
-
-def engine_calls(kind):
-    """Builds and primes bench.py's default engine with every `kind` ('halo' or 'tc') convolution call recorded: returns
-    (mods, {key: (args, kwargs, ConvLayer or None, on the recurrent stage?)})."""
-    import bench
-    from dvmvs import pipeline
-    from dvmvs.fusionnet.model import CostVolumeDecoder, CostVolumeEncoder, FeatureExtractor, FeatureShrinker, LSTMFusion
-    ops.set_conv_backend("tc", terms=1, stride2=True)
-    dev = torch.device(DEV, 0)
-    H, W, D, M = bench.H, bench.W, bench.D, bench.M
-    mods = {"fe": FeatureExtractor(), "fpn": FeatureShrinker(), "cve": CostVolumeEncoder(), "lstm": LSTMFusion(), "cvd": CostVolumeDecoder()}
-    for m in mods.values():
-        shapes = {k: tuple(v.shape) for k, v in m.state_dict().items()}
-        m.load_state_dict({k: torch.from_numpy(v) for k, v in synth.make_state_dict(shapes, seed=7).items()}, strict=True)
-        m.to(dev).eval()
-    clip = [synth.make_clip(0, 1, H, W, M)]
-    ref, rpose, meas, mpose, K = bench.stack_frame(clip, 0)
-    frame = (torch.from_numpy(ref).to(dev), torch.from_numpy(rpose).to(dev), [torch.from_numpy(x).to(dev) for x in meas],
-             [torch.from_numpy(p).to(dev) for p in mpose], torch.from_numpy(K).to(dev))
-    name = "conv2d_halo" if kind == "halo" else "conv2d_tc"
-    real_conv, real_run, real_deferred = getattr(ops, name), ops.ConvLayer.run, ops.ConvLayer.run_deferred
-    calls, current, rec_stream = {}, [], []
-
-    def within(real):
-        def fn(self, *a, **k):
-            current.append(self)
-            try:
-                return real(self, *a, **k)
-            finally:
-                current.pop()
-        return fn
-
-    def record(sources, packed, *a, **kw):
-        key = (id(packed), tuple(sources[0].shape), bool(kw.get("defer_finish")))
-        if key not in calls:
-            on_rec = bool(rec_stream) and torch.cuda.current_stream(dev) == rec_stream[0]
-            calls[key] = ((list(sources), packed) + a, kw, current[-1] if current else None, on_rec)
-        return real_conv(sources, packed, *a, **kw)
-
-    setattr(ops, name, record)
-    ops.ConvLayer.run, ops.ConvLayer.run_deferred = within(real_run), within(real_deferred)
-    try:
-        eng = pipeline.LookaheadFusionnet(mods, batch=1, height=H, width=W, n_measurement_frames=M, n_depth_levels=D, lookahead=4)
-        rec_stream.append(eng.streams[4])
-        with torch.no_grad():
-            eng.prime(*frame)
-        eng.synchronize()
-    finally:
-        setattr(ops, name, real_conv)
-        ops.ConvLayer.run, ops.ConvLayer.run_deferred = real_run, real_deferred
-    return mods, calls
-
-
 def halo_layers(terms):
     import json
-    mods, calls = engine_calls("halo")
+    mods, calls = engine_calls(("conv2d_halo",))
     names = layer_names(mods)
     rows = []
     with torch.no_grad():
@@ -183,7 +115,7 @@ def halo_layers(terms):
 def tc_layers():
     """every conv2d_tc call of the engine (stride 1 and 2, split-K or not, deferred finishing pass or not) replayed alone"""
     import json
-    mods, calls = engine_calls("tc")
+    mods, calls = engine_calls(("conv2d_tc",))
     names = layer_names(mods)
     rows = []
     with torch.no_grad():
