@@ -36,13 +36,15 @@ def _key(name, a, kw):
         return name, tuple(a[1].shape), kw.get("parts") is not None
     if name == "expand_dwconv":
         return name, id(a[1]), tuple(a[0].get_planes().shape)
+    if name == "plane_sweep_tc":          # (reference planes, measurement planes, poses, K, depth range, D); no packed weights
+        return name, tuple(a[0][0].shape), len(a[1]), kw.get("terms")
     return name, id(a[1]), tuple(a[0][0].shape), bool(kw.get("defer_finish"))
 
 
 def engine_calls(ops_recorded=("conv2d_tc",), height=None, width=None, device="cuda"):
     """Builds and primes bench.py's default engine (seed-7 weights, tensor-core backend with 1-term operands; bench.py's input
     size unless height / width are given) with every call of the named functions of dvmvs._ops ("conv2d_tc", "conv2d_halo",
-    "expand_dwconv", "lstm_gates") recorded: returns (mods, {key: (args, kwargs, ConvLayer or None, on the recurrent stage?)}).
+    "expand_dwconv", "lstm_gates", "plane_sweep_tc") recorded: returns (mods, {key: (args, kwargs, ConvLayer or None, on the recurrent stage?)}).
     The recorded tensors are the engine's own buffers: their contents are whatever the engine left in them."""
     import bench
     from dvmvs import pipeline
