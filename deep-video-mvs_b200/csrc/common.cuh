@@ -105,6 +105,17 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
     }                                   \
   } while (0)
 
+#ifdef __CUDACC__
+// x2 bilinear blend (align_corners upsampling) of the four taps with weights ly0/ly1 (rows) and lx0/lx1 (columns).  Every copy of
+// the interpolation (upsample2x_kernel, the fused upsampled conv source, the split / staging kernels) calls this one function, with
+// the roundings spelled out, so that all of them produce the same fp32 value bit for bit whatever the compiler would contract.
+__device__ __forceinline__ float bilerp(float ly0, float ly1, float lx0, float lx1, float v00, float v01, float v10, float v11) {
+  const float top = __fmaf_rn(lx1, v01, __fmul_rn(lx0, v00));
+  const float bot = __fmaf_rn(lx0, v10, __fmul_rn(lx1, v11));
+  return __fmaf_rn(ly0, top, __fmul_rn(ly1, bot));
+}
+#endif
+
 // ---- tiny fp32 linear algebra used by the geometry prologues (device) ---------------------------------
 // Row-major.  The reference does this algebra with torch.inverse / bmm in fp32 on the device
 // (dvmvs/utils.py:51-57,121; dvmvs/convlstm.py:30); any fp32 method agrees to ~1e-7 for rigid poses.

@@ -48,7 +48,7 @@ __device__ __forceinline__ float fetch_src(const dvmvs_conv_desc& d, int s, int 
   const float* base = src + (size_t)b * Hs * Ws * Cs + c;
   const float v00 = __ldg(base + ((size_t)y0 * Ws + x0) * Cs), v01 = __ldg(base + ((size_t)y0 * Ws + x1) * Cs);
   const float v10 = __ldg(base + ((size_t)y1 * Ws + x0) * Cs), v11 = __ldg(base + ((size_t)y1 * Ws + x1) * Cs);
-  return ly0 * (lx0 * v00 + lx1 * v01) + ly1 * (lx0 * v10 + lx1 * v11);
+  return bilerp(ly0, ly1, lx0, lx1, v00, v01, v10, v11);
 }
 
 __device__ __forceinline__ float apply_act(float v, int act) {
@@ -399,7 +399,7 @@ __global__ void upsample2x_kernel(const float* __restrict__ x, float* __restrict
   const float* base = x + (size_t)b * H * W * C + c;
   const float v00 = __ldg(base + ((size_t)y0 * W + x0) * C), v01 = __ldg(base + ((size_t)y0 * W + x1) * C);
   const float v10 = __ldg(base + ((size_t)y1 * W + x0) * C), v11 = __ldg(base + ((size_t)y1 * W + x1) * C);
-  y[idx] = ly0 * (lx0 * v00 + lx1 * v01) + ly1 * (lx0 * v10 + lx1 * v11);
+  y[idx] = bilerp(ly0, ly1, lx0, lx1, v00, v01, v10, v11);
 }
 
 // =====================================================================================================

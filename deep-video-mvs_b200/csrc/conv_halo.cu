@@ -277,9 +277,10 @@ __global__ void __launch_bounds__(kHaloThreads) conv_halo_kernel(const __grid_co
 // [2][B][C8][H'][W'][8] (the C values of x, then zeros); optional x2 bilinear (align_corners) upsampling on the way.
 // hi_only: the lo plane is left unwritten (1-term operands never read it), which halves the bytes stored.
 // One thread per (pixel, 8-channel block): 32-byte reads, one 16-byte store per plane, consecutive threads = consecutive
-// pixels of one channel block (coalesced 512-byte stores per warp).  c_offset must be a multiple of 8.
+// pixels of one channel block (coalesced 512-byte stores per warp).  c_offset must be a multiple of 8.  x_aligned: x is 16-byte
+// aligned, so with C % 4 == 0 every 8-channel block starts on a 16-byte boundary (the host checks; views need not be).
 __global__ void split_blocked_kernel(const float* __restrict__ x, __half* __restrict__ planes, int B, int H, int W, int C, int C8,
-                                     int upsample, int hi_only, int c_offset, int c_cover) {
+                                     int upsample, int hi_only, int c_offset, int c_cover, int x_aligned) {
   pdl_launch_dependents();
   pdl_wait();
   const int Ho = upsample ? 2 * H : H, Wo = upsample ? 2 * W : W;
@@ -296,7 +297,7 @@ __global__ void split_blocked_kernel(const float* __restrict__ x, __half* __rest
   float v[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) v[e] = 0.f;
-  const bool vec = ((C & 3) == 0) && (c0 + 8 <= C);
+  const bool vec = x_aligned && ((C & 3) == 0) && (c0 + 8 <= C);
   if (!upsample) {
     const float* src = x + ((size_t)b * hw + p_in) * C + c0;
     if (vec) {
@@ -330,11 +331,11 @@ __global__ void split_blocked_kernel(const float* __restrict__ x, __half* __rest
       *reinterpret_cast<float4*>(t11) = __ldg(reinterpret_cast<const float4*>(p11));
       *reinterpret_cast<float4*>(t11 + 4) = __ldg(reinterpret_cast<const float4*>(p11 + 4));
 #pragma unroll
-      for (int e = 0; e < 8; ++e) v[e] = ly0 * (lx0 * t00[e] + lx1 * t01[e]) + ly1 * (lx0 * t10[e] + lx1 * t11[e]);
+      for (int e = 0; e < 8; ++e) v[e] = bilerp(ly0, ly1, lx0, lx1, t00[e], t01[e], t10[e], t11[e]);
     } else {
 #pragma unroll
       for (int e = 0; e < 8; ++e)
-        if (c0 + e < C) v[e] = ly0 * (lx0 * __ldg(p00 + e) + lx1 * __ldg(p01 + e)) + ly1 * (lx0 * __ldg(p10 + e) + lx1 * __ldg(p11 + e));
+        if (c0 + e < C) v[e] = bilerp(ly0, ly1, lx0, lx1, __ldg(p00 + e), __ldg(p01 + e), __ldg(p10 + e), __ldg(p11 + e));
     }
   }
   __align__(16) __half hi[8];
@@ -457,8 +458,9 @@ extern "C" int dvmvs_split_blocked(const float* x, void* planes, int B, int H, i
   DVMVS_REQUIRE(c_offset >= 0 && c_cover >= C && c_offset + c_cover <= C8 * 8, "split_blocked: channel window [%d,+%d) outside %d",
                 c_offset, c_cover, C8 * 8);
   DVMVS_REQUIRE(c_offset % 8 == 0, "split_blocked: c_offset must be a multiple of 8 (got %d)", c_offset);
+  DVMVS_REQUIRE((uintptr_t)planes % 16 == 0, "split_blocked: planes must be 16-byte aligned");
   const size_t total = (size_t)B * H * W * ((c_cover + 7) / 8) * (upsample2x ? 4 : 1);
   launch_k(split_blocked_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, (cudaStream_t)stream, x, (__half*)planes, B, H, W, C,
-           C8, upsample2x, (flags & DVMVS_SPLIT_HI_ONLY) ? 1 : 0, c_offset, c_cover);
+           C8, upsample2x, (flags & DVMVS_SPLIT_HI_ONLY) ? 1 : 0, c_offset, c_cover, ((uintptr_t)x % 16 == 0) ? 1 : 0);
   return check_launch("split_blocked_kernel");
 }

@@ -384,8 +384,8 @@ __global__ void split_planes_kernel(const float* __restrict__ x, __half* __restr
       const int y1 = y0 + (y0 < H - 1), x1 = x0 + (x0 < W - 1);
       const float ly1 = fy - y0, lx1 = fx - x0, ly0 = 1.f - ly1, lx0 = 1.f - lx1;
       const float* bp = x + (size_t)b * H * W * C + c;
-      v = ly0 * (lx0 * bp[((size_t)y0 * W + x0) * C] + lx1 * bp[((size_t)y0 * W + x1) * C]) +
-          ly1 * (lx0 * bp[((size_t)y1 * W + x0) * C] + lx1 * bp[((size_t)y1 * W + x1) * C]);
+      v = bilerp(ly0, ly1, lx0, lx1, bp[((size_t)y0 * W + x0) * C], bp[((size_t)y0 * W + x1) * C], bp[((size_t)y1 * W + x0) * C],
+                 bp[((size_t)y1 * W + x1) * C]);
     }
   }
   const __half h = __float2half_rn(v);
@@ -436,7 +436,7 @@ __global__ void split_planes8_kernel(const float* __restrict__ x, __half* __rest
       q = bp + ((size_t)y1 * W + x1) * C;
       *reinterpret_cast<float4*>(t11) = __ldg(reinterpret_cast<const float4*>(q)); *reinterpret_cast<float4*>(t11 + 4) = __ldg(reinterpret_cast<const float4*>(q + 4));
 #pragma unroll
-      for (int e = 0; e < 8; ++e) v[e] = ly0 * (lx0 * t00[e] + lx1 * t01[e]) + ly1 * (lx0 * t10[e] + lx1 * t11[e]);
+      for (int e = 0; e < 8; ++e) v[e] = bilerp(ly0, ly1, lx0, lx1, t00[e], t01[e], t10[e], t11[e]);
     }
   }
   __align__(16) __half hi[8];
