@@ -2,8 +2,11 @@
 pairnet/run-testing.py:139-164) as a function over the drop-in modules, for callers that do not want to copy
 the script's loop body (bench.py, smoke test, examples).  It makes exactly the module / utils calls the script
 makes, with the same keyword arguments."""
+import os
+
 import torch
 
+from . import _native
 from . import _ops as ops
 from ._base import no_auto_graph
 from .utils import (cost_volume_fusion, get_non_differentiable_rectangle_depth_estimation,
@@ -98,6 +101,17 @@ class FeatureCache:
         return idx
 
 
+def _plane_sweep(f2, meas_half, ref_pose, meas_poses, full_K, min_depth, max_depth, n_depth_levels):
+    """Fused plane-sweep cost volume of the reference frame's half-resolution features against the measurement frames'
+    (run-testing.py:161-171), with the intrinsics halved to that resolution.  Returns (cost_volume, half_K)."""
+    half_K = full_K.clone()
+    half_K[:, 0:2, :] = half_K[:, 0:2, :] / 2.0
+    cv = cost_volume_fusion(image1=f2, image2s=meas_half, pose1=ref_pose, pose2s=meas_poses, K=half_K, warp_grid=None,
+                            min_depth=min_depth, max_depth=max_depth, n_depth_levels=n_depth_levels, device=f2.device,
+                            dot_product=True)
+    return cv, half_K
+
+
 def feature_stage(mods, reference_image, reference_pose, measurement_images, measurement_poses, full_K,
                   min_depth=0.25, max_depth=20.0, n_depth_levels=64, batch_features=True, cache=None, reference_id=None,
                   measurement_ids=None):
@@ -108,8 +122,6 @@ def feature_stage(mods, reference_image, reference_pose, measurement_images, mea
     With `cache` (FeatureCache) and frame ids, measurement frames whose half-resolution features are cached skip
     FeatureExtractor + FeatureShrinker (row f1); the reference frame's features are stored under `reference_id`."""
     B = reference_image.shape[0]
-    half_K = full_K.clone()
-    half_K[:, 0:2, :] = half_K[:, 0:2, :] / 2.0
     if cache is not None:
         if measurement_ids is None or len(measurement_ids) != len(measurement_images):
             raise ValueError("feature cache: need one frame id per measurement image")
@@ -134,9 +146,7 @@ def feature_stage(mods, reference_image, reference_pose, measurement_images, mea
             half, _, _, _ = mods["fpn"](*mods["fe"](im))
             meas_half.append(half)
         f2, f4, f8, f16 = mods["fpn"](*mods["fe"](reference_image))
-    cv = cost_volume_fusion(image1=f2, image2s=meas_half, pose1=reference_pose, pose2s=measurement_poses, K=half_K,
-                            warp_grid=None, min_depth=min_depth, max_depth=max_depth, n_depth_levels=n_depth_levels,
-                            device=reference_image.device, dot_product=True)
+    cv, half_K = _plane_sweep(f2, meas_half, reference_pose, measurement_poses, full_K, min_depth, max_depth, n_depth_levels)
     if cache is not None:       # after the sweep: hits are views of ring entries that a store may evict and overwrite
         for m in todo:
             cache.store(measurement_ids[m], meas_half[m])
@@ -145,34 +155,41 @@ def feature_stage(mods, reference_image, reference_pose, measurement_images, mea
     return f2, f4, f8, f16, cv, half_K
 
 
-def recurrent_stage(mods, state, features, reference_image, reference_pose, full_K):
-    """Second half of a keyframe: cost-volume encoder, depth re-projection + ConvLSTM fusion (fusionnet only), decoder
-    (run-testing.py:173-202).  `features` is feature_stage()'s return value.  Returns (depth (B,H,W), state)."""
-    f2, f4, f8, f16, cv, half_K = features
+def _stage_rec(mods, state, slot, enc, half_K):
+    """The loop-carried stage: depth re-projection + ConvLSTM fusion (fusionnet only) and the decoder, from the cost-volume
+    encoder's outputs `enc`.  `slot` holds ref_image, ref_pose and full_K, and optionally what an earlier stage prepared
+    off the loop-carried critical path: ref_cl and lstm_K (_stage_side_inputs), input_gates (_stage_enc)."""
+    s0, s1, s2, s3, bottom = enc
+    reference_image, reference_pose, full_K = slot.get("ref_cl", slot["ref_image"]), slot["ref_pose"], slot["full_K"]
     B, _, H, W = reference_image.shape
-    device = reference_image.device
-    s0, s1, s2, s3, bottom = mods["cve"](features_half=f2, features_quarter=f4, features_one_eight=f8,
-                                         features_one_sixteen=f16, cost_volume=cv)
     if "lstm" in mods:
-        lstm_K = full_K.clone()
-        lstm_K[:, 0:2, :] = lstm_K[:, 0:2, :] / 32.0
+        lstm_K = slot.get("lstm_K")
+        if lstm_K is None:
+            lstm_K = full_K.clone()
+            lstm_K[:, 0:2, :] = lstm_K[:, 0:2, :] / 32.0
         if state.previous_depth is not None:
-            de = get_non_differentiable_rectangle_depth_estimation(reference_pose_torch=reference_pose,
-                                                                   measurement_pose_torch=state.previous_pose,
-                                                                   previous_depth_torch=state.previous_depth,
-                                                                   full_K_torch=full_K, half_K_torch=half_K,
-                                                                   original_height=H, original_width=W)
+            de = get_non_differentiable_rectangle_depth_estimation(reference_pose_torch=reference_pose, measurement_pose_torch=state.previous_pose,
+                                                                   previous_depth_torch=state.previous_depth, full_K_torch=full_K,
+                                                                   half_K_torch=half_K, original_height=H, original_width=W)
             de = de[:, :, ::16, ::16].contiguous()      # == F.interpolate(scale_factor=1/16, mode='nearest') (run-testing.py:187-189)
         else:
-            de = torch.zeros(size=(B, 1, H // 32, W // 32), device=device)
-        state.lstm_state = mods["lstm"](current_encoding=bottom, current_state=state.lstm_state,
-                                        previous_pose=state.previous_pose, current_pose=reference_pose,
-                                        estimated_current_depth=de, camera_matrix=lstm_K)
+            de = torch.zeros(size=(B, 1, H // 32, W // 32), device=reference_image.device)
+        state.lstm_state = mods["lstm"](current_encoding=bottom, current_state=state.lstm_state, previous_pose=state.previous_pose,
+                                        current_pose=reference_pose, estimated_current_depth=de, camera_matrix=lstm_K,
+                                        input_gates=slot.get("input_gates"))
         bottom = state.lstm_state[0]
     pred = mods["cvd"](reference_image, s0, s1, s2, s3, bottom)[0]
     state.previous_depth = pred.view(B, 1, H, W)
     state.previous_pose = reference_pose
     return pred, state
+
+
+def recurrent_stage(mods, state, features, reference_image, reference_pose, full_K):
+    """Second half of a keyframe: cost-volume encoder, depth re-projection + ConvLSTM fusion (fusionnet only), decoder
+    (run-testing.py:173-202).  `features` is feature_stage()'s return value.  Returns (depth (B,H,W), state)."""
+    f2, f4, f8, f16, cv, half_K = features
+    enc = mods["cve"](features_half=f2, features_quarter=f4, features_one_eight=f8, features_one_sixteen=f16, cost_volume=cv)
+    return _stage_rec(mods, state, {"ref_image": reference_image, "ref_pose": reference_pose, "full_K": full_K}, enc, half_K)
 
 
 def keyframe(mods, state, reference_image, reference_pose, measurement_images, measurement_poses, full_K,
@@ -189,6 +206,118 @@ def keyframe(mods, state, reference_image, reference_pose, measurement_images, m
     return recurrent_stage(mods, state, feats, reference_image, reference_pose, full_K)
 
 
+class _StaticState:
+    """The recurrent state in static device buffers that the captured graphs of the loop-carried stage read and rewrite.
+    The only code that knows the buffers' order: h, c, previous depth (B,1,H,W), previous pose."""
+
+    def __init__(self):
+        self.buffers = None       # allocated from the first recurrent result
+
+    def allocate(self, state):
+        self.buffers = (state.lstm_state[0].clone(), state.lstm_state[1].clone(), state.previous_depth.clone(),
+                        state.previous_pose.clone())
+
+    def keyframe_state(self, with_state):
+        """A fresh KeyframeState; with_state: over views of the static buffers."""
+        st = KeyframeState()
+        if with_state:
+            h, c, pd, pp = self.buffers
+            st.lstm_state, st.previous_depth, st.previous_pose = (h, c), pd, pp
+        return st
+
+    def load(self, lstm_state, previous_depth, previous_pose):
+        h, c, pd, pp = self.buffers
+        with torch.no_grad():
+            h.copy_(lstm_state[0])
+            c.copy_(lstm_state[1])
+            pd.copy_(previous_depth.reshape(pd.shape))
+            pp.copy_(previous_pose)
+
+    def write_back(self, state):
+        """New recurrent state -> static buffers (read by the next replay)."""
+        self.load(state.lstm_state, state.previous_depth, state.previous_pose)
+
+    def snapshot(self):
+        return None if self.buffers is None else [t.clone() for t in self.buffers]
+
+    def restore(self, saved):
+        if saved is not None:
+            for dst, src in zip(self.buffers, saved):
+                dst.copy_(src)
+
+
+def _capture_graph(fn, stream, pdl=None, state=None, depth=None):
+    """Warms `fn` up twice on `stream` (allocations, weight packing, function attributes), then captures it there.
+    Returns (graph, result of the captured run, kernels of ours in the graph).
+
+    pdl: None keeps the library's programmatic-dependent-launch default, False / True force it off / on for the
+    warm-ups and the capture.  `state` (_StaticState) marks the loop-carried stage, whose fn returns (depth, KeyframeState):
+    the graph then ends with the copy of the depth into `depth` and of the new state into the static buffers, which are
+    allocated from the warm-up's result if need be; the state the buffers held before is put back afterwards."""
+    saved = state.snapshot() if state is not None else None
+    if pdl is not None:
+        _native.lib().dvmvs_set_programmatic_launch(int(pdl))
+    try:
+        with torch.cuda.stream(stream), torch.no_grad(), no_auto_graph():
+            for _ in range(2):
+                res = fn()
+        stream.synchronize()
+        if state is not None and state.buffers is None:
+            state.allocate(res[1])
+        g = torch.cuda.CUDAGraph()
+        n0 = _native.launch_count()
+        with torch.no_grad(), torch.cuda.graph(g, stream=stream):
+            res = fn()
+            if state is not None:
+                depth.copy_(res[0])
+                state.write_back(res[1])
+        n = _native.launch_count() - n0
+    finally:
+        if pdl is not None:
+            _native.lib().dvmvs_set_programmatic_launch(-1)
+    if state is not None:
+        state.restore(saved)
+    return g, res, n
+
+
+def _after_caller(first, last, device, frame, out):
+    """The inputs were produced on the caller's stream: orders the engine's first stream after it and keeps CUDA inputs
+    (and a CUDA `out`, written on the last stream) alive, caching-allocator wise, until the engine's work on them has run."""
+    reference_image, reference_pose, measurement_images, measurement_poses, full_K = frame
+    first.wait_stream(torch.cuda.current_stream(device))
+    for t_in in [reference_image, reference_pose, full_K] + list(measurement_images) + list(measurement_poses):
+        if t_in is not None and t_in.is_cuda:
+            t_in.record_stream(first)
+    if out is not None and out.is_cuda:
+        out.record_stream(last)
+
+
+def _upload(slot, frame, hits=None):
+    """Copies one keyframe's inputs (CPU-pinned or CUDA) into the static buffers of `slot` on the current stream.
+    hits[m]: the feature cache holds measurement frame m, which then needs no image."""
+    reference_image, reference_pose, measurement_images, measurement_poses, full_K = frame
+    slot["ref_image"].copy_(reference_image, non_blocking=True)
+    slot["ref_pose"].copy_(reference_pose, non_blocking=True)
+    slot["full_K"].copy_(full_K, non_blocking=True)
+    for m, (dst, src) in enumerate(zip(slot["meas_images"], measurement_images)):
+        if hits is None or not hits[m]:
+            dst.copy_(src, non_blocking=True)
+    for dst, src in zip(slot["meas_poses"], measurement_poses):
+        dst.copy_(src, non_blocking=True)
+
+
+def _load_state(self, lstm_state, previous_depth, previous_pose):
+    """Continue a clip whose first keyframes ran elsewhere (e.g. through the module calls with fewer measurement frames):
+    installs (h, c), the previous depth (B,1,H,W) and the previous pose as the recurrent state of the next submit().
+    Needs the static state buffers, i.e. prime() or one earlier keyframe."""
+    if self._static_state.buffers is None:
+        raise RuntimeError("load_state: call prime() (or submit one keyframe) first")
+    self.synchronize()
+    self._static_state.load(lstm_state, previous_depth, previous_pose)
+    torch.cuda.current_stream(self.device).synchronize()
+    self._has_state = True
+
+
 class GraphedFusionnet:
     """The keyframe loop body captured once into CUDA graphs (static shapes) and replayed: removes the ~300 host-side
     launches per keyframe.  Built from the same drop-in modules; two graphs are captured lazily -- keyframe without
@@ -203,87 +332,51 @@ class GraphedFusionnet:
     def __init__(self, mods, batch, height, width, n_measurement_frames, min_depth=0.25, max_depth=20.0, n_depth_levels=64,
                  device=None):
         self.mods, self.B, self.H, self.W, self.M = mods, batch, height, width, n_measurement_frames
-        self.min_depth, self.max_depth, self.D = min_depth, max_depth, n_depth_levels
+        self.depth_args = (min_depth, max_depth, n_depth_levels)
         dev = device or next(mods["fe"].parameters()).device
         self.device = dev
         z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
-        self.ref_image, self.ref_pose, self.full_K = z(batch, 3, height, width), z(batch, 4, 4), z(batch, 3, 3)
-        self.meas_images = [z(batch, 3, height, width) for _ in range(n_measurement_frames)]
-        self.meas_poses = [z(batch, 4, 4) for _ in range(n_measurement_frames)]
+        self.slot = {"ref_image": z(batch, 3, height, width), "ref_pose": z(batch, 4, 4), "full_K": z(batch, 3, 3),
+                     "meas_images": [z(batch, 3, height, width) for _ in range(n_measurement_frames)],
+                     "meas_poses": [z(batch, 4, 4) for _ in range(n_measurement_frames)]}
         self.state = KeyframeState()
         self._graphs = {}
         self._capture_stream = None
         self.kernels_per_replay = {}
-        self._static_state = None     # (h, c, prev_depth, prev_pose) buffers the steady-state graph reads and rewrites
-        self._out = None
+        self._static_state = _StaticState()
+        self._out = z(batch, height, width)
         self._has_state = False
 
     def reset(self):
         self._has_state = False
 
-    def _load_inputs(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K):
-        self.ref_image.copy_(reference_image, non_blocking=True)
-        self.ref_pose.copy_(reference_pose, non_blocking=True)
-        self.full_K.copy_(full_K, non_blocking=True)
-        for dst, src in zip(self.meas_images, measurement_images):
-            dst.copy_(src, non_blocking=True)
-        for dst, src in zip(self.meas_poses, measurement_poses):
-            dst.copy_(src, non_blocking=True)
-
     def _body(self, with_state):
-        st = KeyframeState()
-        if with_state:
-            h, c, pd, pp = self._static_state
-            st.lstm_state, st.previous_depth, st.previous_pose = (h, c), pd, pp
-        pred, st = keyframe(self.mods, st, self.ref_image, self.ref_pose, self.meas_images, self.meas_poses, self.full_K,
-                            self.min_depth, self.max_depth, self.D)
-        return pred, st
+        slot = self.slot
+        return keyframe(self.mods, self._static_state.keyframe_state(with_state), slot["ref_image"], slot["ref_pose"],
+                        slot["meas_images"], slot["meas_poses"], slot["full_K"], *self.depth_args)
 
     def _capture(self, with_state):
-        # warm-up on a side stream (allocations, weight packing, function attributes), then capture
         if self._capture_stream is None:
             self._capture_stream = torch.cuda.Stream(device=self.device)
         s = self._capture_stream        # same stream for warm-up and capture: per-stream scratch is allocated outside the graph
-        s.wait_stream(torch.cuda.current_stream(self.device))
-        with torch.cuda.stream(s), torch.no_grad(), no_auto_graph():
-            for _ in range(2):
-                pred, st = self._body(with_state)
-        torch.cuda.current_stream(self.device).wait_stream(s)
-        s.synchronize()
-        if self._static_state is None:
-            self._static_state = (st.lstm_state[0].clone(), st.lstm_state[1].clone(), st.previous_depth.clone(), self.ref_pose.clone())
-            self._out = torch.empty_like(pred)
-        from . import _native
-        g = torch.cuda.CUDAGraph()
-        n0 = _native.launch_count()
-        with torch.no_grad(), torch.cuda.graph(g, stream=s):
-            pred, st = self._body(with_state)
-            self.kernels_per_replay[with_state] = _native.launch_count() - n0   # our kernels captured in this graph
-            h, c, pd, pp = self._static_state
-            self._out.copy_(pred)
-            # new recurrent state -> static buffers (read by the next replay)
-            h.copy_(st.lstm_state[0])
-            c.copy_(st.lstm_state[1])
-            pd.copy_(st.previous_depth)
-            pp.copy_(self.ref_pose)
-        self._graphs[with_state] = g
+        caller = torch.cuda.current_stream(self.device)
+        s.wait_stream(caller)
+        with torch.cuda.stream(s):      # the snapshot and the restore of the recurrent state around the warm-ups run on s too
+            self._graphs[with_state], _, self.kernels_per_replay[with_state] = _capture_graph(
+                lambda: self._body(with_state), s, None, self._static_state, self._out)
+        caller.wait_stream(s)
 
     def step(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K):
         if len(measurement_images) != self.M:
             raise ValueError("GraphedFusionnet was built for %d measurement frames, got %d" % (self.M, len(measurement_images)))
+        frame = (reference_image, reference_pose, measurement_images, measurement_poses, full_K)
         with_state = self._has_state
         if with_state not in self._graphs:
-            if with_state and self._static_state is None:
+            if with_state and self._static_state.buffers is None:
                 raise RuntimeError("steady-state graph requested before any keyframe ran")
-            saved = None
-            if self._static_state is not None:
-                saved = [t.clone() for t in self._static_state]
-            self._load_inputs(reference_image, reference_pose, measurement_images, measurement_poses, full_K)
+            _upload(self.slot, frame)
             self._capture(with_state)
-            if saved is not None:                      # capture warm-ups must not advance the recurrent state
-                for dst, src in zip(self._static_state, saved):
-                    dst.copy_(src)
-        self._load_inputs(reference_image, reference_pose, measurement_images, measurement_poses, full_K)
+        _upload(self.slot, frame)
         self._graphs[with_state].replay()
         self._has_state = True
         return self._out
@@ -292,7 +385,6 @@ class GraphedFusionnet:
 def _stage_side_inputs(slot):
     """Small state-independent preparations the last stage would otherwise do on the loop-carried critical path: the
     channel-last copy of the reference image the decoder's refinement convolutions read, and the 1/32 intrinsics."""
-    from . import _ops as ops
     slot["ref_cl"] = ops.to_api(ops.to_nhwc(slot["ref_image"], "image"))      # (B,3,H,W) view with channels_last strides
     lstm_K = slot["full_K"].clone()
     lstm_K[:, 0:2, :] = lstm_K[:, 0:2, :] / 32.0
@@ -337,10 +429,7 @@ def _sweep_from_pyramid(slot, pyramid, base, min_depth, max_depth, n_depth_level
     else:
         f2, f4, f8, f16 = ops.batch_slice(a2, base, base + B), a4[base:base + B], a8[base:base + B], a16[base:base + B]
         meas_half = [ops.batch_slice(a2, base + (m + 1) * B, base + (m + 2) * B) for m in range(M)]
-    half_K = slot["full_K"].clone()
-    half_K[:, 0:2, :] = half_K[:, 0:2, :] / 2.0
-    cv = cost_volume_fusion(image1=f2, image2s=meas_half, pose1=slot["ref_pose"], pose2s=slot["meas_poses"], K=half_K, warp_grid=None,
-                            min_depth=min_depth, max_depth=max_depth, n_depth_levels=n_depth_levels, device=f2.device, dot_product=True)
+    cv, half_K = _plane_sweep(f2, meas_half, slot["ref_pose"], slot["meas_poses"], slot["full_K"], min_depth, max_depth, n_depth_levels)
     return (f2, f4, f8, f16, cv), half_K
 
 
@@ -363,29 +452,23 @@ def _stage_mid(mods, slot, fe_out, min_depth, max_depth, n_depth_levels):
     return _stage_enc(mods, slot, _stage_sweep(mods, slot, fe_out, min_depth, max_depth, n_depth_levels))
 
 
-def _stage_rec(mods, state, slot, enc, half_K):
-    """Last stage: depth re-projection + ConvLSTM fusion + decoder -- the only part with a loop-carried dependence."""
-    s0, s1, s2, s3, bottom = enc
-    reference_image, reference_pose, full_K = slot.get("ref_cl", slot["ref_image"]), slot["ref_pose"], slot["full_K"]
-    B, _, H, W = reference_image.shape
-    lstm_K = slot.get("lstm_K")
-    if lstm_K is None:
-        lstm_K = full_K.clone()
-        lstm_K[:, 0:2, :] = lstm_K[:, 0:2, :] / 32.0
-    if state.previous_depth is not None:
-        de = get_non_differentiable_rectangle_depth_estimation(reference_pose_torch=reference_pose, measurement_pose_torch=state.previous_pose,
-                                                               previous_depth_torch=state.previous_depth, full_K_torch=full_K,
-                                                               half_K_torch=half_K, original_height=H, original_width=W)
-        de = de[:, :, ::16, ::16].contiguous()
-    else:
-        de = torch.zeros(size=(B, 1, H // 32, W // 32), device=reference_image.device)
-    state.lstm_state = mods["lstm"](current_encoding=bottom, current_state=state.lstm_state, previous_pose=state.previous_pose,
-                                    current_pose=reference_pose, estimated_current_depth=de, camera_matrix=lstm_K,
-                                    input_gates=slot.get("input_gates"))
-    pred = mods["cvd"](reference_image, s0, s1, s2, s3, state.lstm_state[0])[0]
-    state.previous_depth = pred.view(B, 1, H, W)
-    state.previous_pose = reference_pose
-    return pred, state
+# PipelinedFusionnet's stages, each called as fn(engine, slot, output of the previous stage, recurrent state), and its plans.
+# Only the last stage of a plan reads the recurrent state; everything before it is independent of the previous keyframe.
+_STAGES = {
+    "features": lambda e, slot, prev, st: feature_stage(e.mods, slot["ref_image"], slot["ref_pose"], slot["meas_images"],
+                                                        slot["meas_poses"], slot["full_K"], *e.depth_args),
+    "fe": lambda e, slot, prev, st: _stage_fe(e.mods, slot),
+    "head": lambda e, slot, prev, st: _stage_fe_head(e.mods, slot),
+    "tail": lambda e, slot, prev, st: _stage_fe_tail(e.mods, slot, prev),
+    "mid": lambda e, slot, prev, st: _stage_mid(e.mods, slot, prev, *e.depth_args),
+    "sweep": lambda e, slot, prev, st: _stage_sweep(e.mods, slot, prev, *e.depth_args),
+    "enc": lambda e, slot, prev, st: _stage_enc(e.mods, slot, prev),
+    "rec": lambda e, slot, prev, st: _stage_rec(e.mods, st, slot, *prev),
+    "enc+rec": lambda e, slot, prev, st: recurrent_stage(e.mods, st, prev, slot["ref_image"], slot["ref_pose"], slot["full_K"]),
+}
+_PLANS = {2: ("features", "enc+rec"), 3: ("fe", "mid", "rec"), 4: ("head", "tail", "mid", "rec"),
+          5: ("head", "tail", "sweep", "enc", "rec")}
+_SWEEP_STAGES = ("features", "mid", "sweep")      # the stages that hold FPN + plane sweep
 
 
 class PipelinedFusionnet:
@@ -405,12 +488,12 @@ class PipelinedFusionnet:
 
     def __init__(self, mods, batch, height, width, n_measurement_frames, min_depth=0.25, max_depth=20.0, n_depth_levels=64,
                  device=None, n_stages=3, feature_cache=0):
-        if n_stages not in (2, 3, 4, 5):
+        if n_stages not in _PLANS:
             raise ValueError("n_stages must be 2, 3, 4 or 5")
         if feature_cache and n_stages < 3:
             raise ValueError("the feature cache needs n_stages >= 3 (feature pyramid + plane sweep in one stage)")
         self.mods, self.B, self.H, self.W, self.M = mods, batch, height, width, n_measurement_frames
-        self.min_depth, self.max_depth, self.D = min_depth, max_depth, n_depth_levels
+        self.depth_args = (min_depth, max_depth, n_depth_levels)
         dev = device or next(mods["fe"].parameters()).device
         self.device = dev
         self.n_stages = n_stages
@@ -430,23 +513,23 @@ class PipelinedFusionnet:
         if self.cache is not None:
             for slot in self.slots:
                 slot["meas_half"] = [z(batch, height // 2, width // 2, 32) for _ in range(n_measurement_frames)]
-        self._sweep_stage = {2: 0, 3: 1, 4: 2, 5: 2}[n_stages]      # the stage that holds FPN + plane sweep
-        import os as _os
+        self._plan = _PLANS[n_stages]
+        self._sweep_stage = next(i for i, kind in enumerate(self._plan) if kind in _SWEEP_STAGES)
         # DVMVS_PIPE_PRIO=1 gives the last stage (the one carrying the loop dependence) a high-priority stream; measured
         # slower on the previous architecture, so it is off by default
-        prio = _os.environ.get("DVMVS_PIPE_PRIO", "0") == "1"
+        prio = os.environ.get("DVMVS_PIPE_PRIO", "0") == "1"
         self.streams = [torch.cuda.Stream(device=dev, priority=(-1 if (prio and i == n_stages - 1) else 0)) for i in range(n_stages)]
         # DVMVS_PIPE_REC_PDL=0: capture the last stage without programmatic dependent launch (its early-launched CTAs then do
         # not sit on SMs waiting for their predecessor while other stages could use them) -- experiment switch
-        self._rec_pdl = _os.environ.get("DVMVS_PIPE_REC_PDL", "1") == "1"
+        self._rec_pdl = os.environ.get("DVMVS_PIPE_REC_PDL", "1") == "1"
         # DVMVS_PIPE_PDL=1: capture the stages WITH programmatic dependent launch.  Off by default: with several stage graphs in
         # flight, early-launched CTAs that sit in griddepcontrol.wait hold shared memory and SM slots other stages' kernels
         # could use (measured slower with 5 stages on the previous architecture; a stage replayed alone gains a little from it)
-        self._pdl = _os.environ.get("DVMVS_PIPE_PDL", "0") == "1"
-        if _os.environ.get("DVMVS_PIPE_SERIAL") == "1":        # debugging aid: all stages on one stream (no overlap)
+        self._pdl = os.environ.get("DVMVS_PIPE_PDL", "0") == "1"
+        if os.environ.get("DVMVS_PIPE_SERIAL") == "1":        # debugging aid: all stages on one stream (no overlap)
             self.streams = [self.streams[0]] * n_stages
         self.stream_a, self.stream_b = self.streams[0], self.streams[-1]      # first / last stage (timing hooks)
-        self._static_state = None
+        self._static_state = _StaticState()
         self._has_state = False
         self.t = 0
         self._kernels = [0] * n_stages
@@ -456,94 +539,20 @@ class PipelinedFusionnet:
         """TRACKING LOST / new clip: drops the recurrent state (the feature cache is keyed by frame id and stays valid)."""
         self._has_state = False
 
-    def load_state(self, lstm_state, previous_depth, previous_pose):
-        """Continue a clip whose first keyframes ran elsewhere (e.g. through the module calls with fewer measurement frames):
-        installs (h, c), the previous depth (B,1,H,W) and the previous pose as the recurrent state of the next submit().
-        Needs the static state buffers, i.e. prime() or one earlier keyframe."""
-        if self._static_state is None:
-            raise RuntimeError("load_state: call prime() (or submit one keyframe) first")
-        self.synchronize()
-        h, c, pd, pp = self._static_state
-        with torch.no_grad():
-            h.copy_(lstm_state[0])
-            c.copy_(lstm_state[1])
-            pd.copy_(previous_depth.reshape(pd.shape))
-            pp.copy_(previous_pose)
-        torch.cuda.current_stream(self.device).synchronize()
-        self._has_state = True
+    load_state = _load_state
 
-    # -- stage bodies -----------------------------------------------------------------------------------------------
     def _run_stage(self, i, slot, with_state):
-        last = self.n_stages - 1
-        prev = slot["out"][i - 1] if i > 0 else None
-        depth_args = (self.min_depth, self.max_depth, self.D)
-        if self.n_stages == 2:
-            if i == 0:
-                return feature_stage(self.mods, slot["ref_image"], slot["ref_pose"], slot["meas_images"], slot["meas_poses"],
-                                     slot["full_K"], self.min_depth, self.max_depth, self.D)
-        elif i < last:
-            # stage plans (all stages before the last are independent of the recurrent state):
-            #   3: FE | FPN + sweep + encoder | rec        4: FE head | FE tail | FPN + sweep + encoder | rec
-            #   5: FE head | FE tail | FPN + sweep | encoder | rec
-            plan = {3: ("fe", "mid"), 4: ("head", "tail", "mid"), 5: ("head", "tail", "sweep", "enc")}[self.n_stages]
-            kind = plan[i]
-            if kind == "fe":
-                return _stage_fe(self.mods, slot)
-            if kind == "head":
-                return _stage_fe_head(self.mods, slot)
-            if kind == "tail":
-                return _stage_fe_tail(self.mods, slot, prev)
-            if kind == "mid":
-                return _stage_mid(self.mods, slot, prev, *depth_args)
-            if kind == "sweep":
-                return _stage_sweep(self.mods, slot, prev, *depth_args)
-            return _stage_enc(self.mods, slot, prev)
-        st = KeyframeState()
-        if with_state:
-            h, c, pd, pp = self._static_state
-            st.lstm_state, st.previous_depth, st.previous_pose = (h, c), pd, pp
-        if self.n_stages == 2:
-            return recurrent_stage(self.mods, st, slot["out"][0], slot["ref_image"], slot["ref_pose"], slot["full_K"])
-        enc, half_K = slot["out"][last - 1]
-        return _stage_rec(self.mods, st, slot, enc, half_K)
+        return _STAGES[self._plan[i]](self, slot, slot["out"][i - 1] if i > 0 else None, self._static_state.keyframe_state(with_state))
 
     def _capture(self, i, slot, with_state):
-        from . import _native
-        last = self.n_stages - 1
-        stream = self.streams[i]
+        last = i == self.n_stages - 1
+        pdl_off = (not self._pdl) or (last and not self._rec_pdl)
         torch.cuda.synchronize(self.device)
-        saved = [t.clone() for t in self._static_state] if (i == last and self._static_state is not None) else None
-        pdl_off = (not self._pdl) or (i == last and not self._rec_pdl)
-        if pdl_off:
-            _native.lib().dvmvs_set_programmatic_launch(0)
-        with torch.cuda.stream(stream), torch.no_grad(), no_auto_graph():
-            for _ in range(2):
-                res = self._run_stage(i, slot, with_state)
-        stream.synchronize()
-        if i == last and self._static_state is None:
-            pred, st = res
-            self._static_state = (st.lstm_state[0].clone(), st.lstm_state[1].clone(), st.previous_depth.clone(), slot["ref_pose"].clone())
-        g = torch.cuda.CUDAGraph()
-        n0 = _native.launch_count()
-        with torch.no_grad(), torch.cuda.graph(g, stream=stream):
-            res = self._run_stage(i, slot, with_state)
-            if i == last:
-                pred, st = res
-                h, c, pd, pp = self._static_state
-                slot["depth"].copy_(pred)
-                h.copy_(st.lstm_state[0])
-                c.copy_(st.lstm_state[1])
-                pd.copy_(st.previous_depth)
-                pp.copy_(slot["ref_pose"])
-            else:
-                slot["out"][i] = res
-        self._kernels[i] = _native.launch_count() - n0
-        if pdl_off:
-            _native.lib().dvmvs_set_programmatic_launch(-1)
-        slot["graph"][i][with_state if i == last else False] = g
-        if saved is not None:
-            for dst, src in zip(self._static_state, saved):
-                dst.copy_(src)
+        g, res, self._kernels[i] = _capture_graph(lambda: self._run_stage(i, slot, with_state), self.streams[i],
+                                                  False if pdl_off else None, *((self._static_state, slot["depth"]) if last else ()))
+        if not last:
+            slot["out"][i] = res
+        slot["graph"][i][with_state if last else False] = g
         torch.cuda.synchronize(self.device)
 
     # -- steady state ----------------------------------------------------------------------------------------------
@@ -570,29 +579,15 @@ class PipelinedFusionnet:
                     raise ValueError("feature cache miss for frame id %r and no image given" % (measurement_ids[m],))
         elif reference_id is not None or measurement_ids is not None:
             raise ValueError("frame ids given but the engine was built without feature_cache")
-        # the inputs were produced on the caller's stream: order the first stage after it and keep CUDA inputs alive
-        # (caching-allocator wise) until our copies on the stage stream have run
-        caller = torch.cuda.current_stream(self.device)
-        self.streams[0].wait_stream(caller)
-        for t_in in [reference_image, reference_pose, full_K] + list(measurement_images) + list(measurement_poses):
-            if t_in is not None and t_in.is_cuda:
-                t_in.record_stream(self.streams[0])
-        if out is not None and out.is_cuda:
-            out.record_stream(self.streams[last])
+        frame = (reference_image, reference_pose, measurement_images, measurement_poses, full_K)
+        _after_caller(self.streams[0], self.streams[last], self.device, frame, out)
         for i in range(n):
             stream = self.streams[i]
             key = with_state if i == last else False
             with torch.cuda.stream(stream):
                 if i == 0:
                     stream.wait_event(slot["done"][last])         # slot reuse: keyframe t-n has left the pipeline
-                    slot["ref_image"].copy_(reference_image, non_blocking=True)
-                    slot["ref_pose"].copy_(reference_pose, non_blocking=True)
-                    slot["full_K"].copy_(full_K, non_blocking=True)
-                    for m, (dst, src) in enumerate(zip(slot["meas_images"], measurement_images)):
-                        if hits is None or not hits[m]:            # cached measurement frames need no image upload
-                            dst.copy_(src, non_blocking=True)
-                    for dst, src in zip(slot["meas_poses"], measurement_poses):
-                        dst.copy_(src, non_blocking=True)
+                    _upload(slot, frame, hits)
                 else:
                     stream.wait_event(slot["done"][i - 1])
                 if hits is not None and i == self._sweep_stage:
@@ -681,7 +676,7 @@ class LookaheadFusionnet:
         if lookahead < 1 or n_groups < 2:
             raise ValueError("lookahead >= 1 and n_groups >= 2 required")
         self.mods, self.B, self.H, self.W, self.M = mods, batch, height, width, n_measurement_frames
-        self.min_depth, self.max_depth, self.D = min_depth, max_depth, n_depth_levels
+        self.depth_args = (min_depth, max_depth, n_depth_levels)
         dev = device or next(mods["fe"].parameters()).device
         self.device = dev
         self.T, self.G = int(lookahead), int(n_groups)
@@ -706,16 +701,13 @@ class LookaheadFusionnet:
                                     "depth": z(batch, height, width), "graph": dict(), "done": torch.cuda.Event()})
         # the recurrent stage's small kernels carry the loop dependence; on a high-priority stream their CTAs are dispatched
         # ahead of the queued CTAs of the batched stages' big grids (DVMVS_LA_PRIO=0: all streams equal)
-        import os as _os
-        prio = _os.environ.get("DVMVS_LA_PRIO", "1") == "1"
-        # experiment switches, both off: DVMVS_LA_FOREACH=1 writes the recurrent state back with one multi-tensor copy instead of
-        # five copy kernels (no gain measured); DVMVS_LA_REC_PDL=1 captures the recurrent stage's graph with programmatic dependent
-        # launch (measured slower, as for the other stages)
-        self._foreach = _os.environ.get("DVMVS_LA_FOREACH", "0") == "1" and hasattr(torch, "_foreach_copy_")
-        self._rec_pdl = _os.environ.get("DVMVS_LA_REC_PDL", "0") == "1"
+        prio = os.environ.get("DVMVS_LA_PRIO", "1") == "1"
+        # experiment switch, off: DVMVS_LA_REC_PDL=1 captures the recurrent stage's graph with programmatic dependent launch
+        # (measured slower, as for the other stages)
+        self._rec_pdl = os.environ.get("DVMVS_LA_REC_PDL", "0") == "1"
         self.streams = [torch.cuda.Stream(device=dev, priority=(-1 if (prio and i == 4) else 0)) for i in range(5)]
         self.stream_a, self.stream_b = self.streams[0], self.streams[-1]
-        self._static_state = None
+        self._static_state = _StaticState()
         self._has_state = False
         self._gi, self._fill = 0, 0          # group counter, keyframes buffered in the open group
         self._pending = []                   # (kslot index, with_state, out) of the open group
@@ -728,73 +720,26 @@ class LookaheadFusionnet:
         """New clip / tracking lost: the next submitted keyframe starts without recurrent state (buffered keyframes keep theirs)."""
         self._has_state = False
 
-    def load_state(self, lstm_state, previous_depth, previous_pose):
-        """As PipelinedFusionnet.load_state: continue a clip whose first keyframes ran elsewhere."""
-        if self._static_state is None:
-            raise RuntimeError("load_state: call prime() (or submit one keyframe) first")
-        self.synchronize()
-        h, c, pd, pp = self._static_state
-        with torch.no_grad():
-            h.copy_(lstm_state[0])
-            c.copy_(lstm_state[1])
-            pd.copy_(previous_depth.reshape(pd.shape))
-            pp.copy_(previous_pose)
-        torch.cuda.current_stream(self.device).synchronize()
-        self._has_state = True
+    load_state = _load_state
 
-    # -- capture helpers ------------------------------------------------------------------------------------------------
-    def _graph_of(self, fn, stream, rec=False):
-        """Warm up `fn` twice on `stream`, capture it; returns (graph, result of the captured run, kernels launched)."""
-        from . import _native
+    def _capture(self, fn, stream, ks=None):
+        """Graph of one of a group's batched stages, or (`ks`) of the recurrent stage of keyframe slot `ks`; returns what
+        _capture_graph returns.  No PDL: it costs throughput with stages in flight (see PipelinedFusionnet)."""
         torch.cuda.synchronize(self.device)
-        saved = [t.clone() for t in self._static_state] if (rec and self._static_state is not None) else None
-        _native.lib().dvmvs_set_programmatic_launch(1 if (rec and self._rec_pdl) else 0)   # see PipelinedFusionnet: PDL costs throughput with stages in flight
-        try:
-            with torch.cuda.stream(stream), torch.no_grad(), no_auto_graph():
-                for _ in range(2):
-                    res = fn()
-            stream.synchronize()
-            if rec and self._static_state is None:
-                pred, st = res
-                self._static_state = (st.lstm_state[0].clone(), st.lstm_state[1].clone(), st.previous_depth.clone(), st.previous_pose.clone())
-            g = torch.cuda.CUDAGraph()
-            n0 = _native.launch_count()
-            with torch.no_grad(), torch.cuda.graph(g, stream=stream):
-                res = fn(capturing=True) if rec else fn()
-            n = _native.launch_count() - n0
-        finally:
-            _native.lib().dvmvs_set_programmatic_launch(-1)
-        if saved is not None:
-            for dst, src in zip(self._static_state, saved):
-                dst.copy_(src)
+        captured = _capture_graph(fn, stream, ks is not None and self._rec_pdl,
+                                  *((self._static_state, ks["depth"]) if ks is not None else ()))
         torch.cuda.synchronize(self.device)
-        return g, res, n
+        return captured
 
-    def _rec_fn(self, ks, grp, with_state):
+    def _run_rec(self, ks, grp, with_state):
         lo, hi = ks["lo"], ks["hi"]
-
-        def fn(capturing=False):
-            st = KeyframeState()
-            if with_state:
-                h, c, pd, pp = self._static_state
-                st.lstm_state, st.previous_depth, st.previous_pose = (h, c), pd, pp
-            enc, half_K = grp["enc"]
-            view = {"ref_image": ks["ref_image"], "ref_pose": ks["ref_pose"], "full_K": ks["full_K"], "ref_cl": grp["ref_cl"][lo:hi],
-                    "lstm_K": grp["lstm_K"][lo:hi]}
-            if grp.get("input_gates") is not None:
-                view["input_gates"] = grp["input_gates"][lo:hi]
-            pred, st = _stage_rec(self.mods, st, view, tuple(ops.batch_slice(e, lo, hi) for e in enc), half_K[lo:hi])
-            if capturing:
-                h, c, pd, pp = self._static_state
-                dsts = [ks["depth"], h, c, pd, pp]
-                srcs = [pred, st.lstm_state[0], st.lstm_state[1], st.previous_depth.reshape(pd.shape), ks["ref_pose"]]
-                if self._foreach:        # one multi-tensor launch instead of five copy kernels at the end of the loop-carried chain
-                    torch._foreach_copy_(dsts, [s_.reshape(d_.shape) for d_, s_ in zip(dsts, srcs)])
-                else:
-                    for d_, s_ in zip(dsts, srcs):
-                        d_.copy_(s_)
-            return pred, st
-        return fn
+        enc, half_K = grp["enc"]
+        view = {"ref_image": ks["ref_image"], "ref_pose": ks["ref_pose"], "full_K": ks["full_K"], "ref_cl": grp["ref_cl"][lo:hi],
+                "lstm_K": grp["lstm_K"][lo:hi]}
+        if grp.get("input_gates") is not None:
+            view["input_gates"] = grp["input_gates"][lo:hi]
+        return _stage_rec(self.mods, self._static_state.keyframe_state(with_state), view,
+                          tuple(ops.batch_slice(e, lo, hi) for e in enc), half_K[lo:hi])
 
     # -- steady state ---------------------------------------------------------------------------------------------------
     def submit(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K, out=None):
@@ -803,25 +748,13 @@ class LookaheadFusionnet:
         g = self._gi % self.G
         grp = self.groups[g]
         ki = g * self.T + self._fill
-        ks = self.kslots[ki]
         s0 = self.streams[0]
-        caller = torch.cuda.current_stream(self.device)
-        s0.wait_stream(caller)
-        for t_in in [reference_image, reference_pose, full_K] + list(measurement_images) + list(measurement_poses):
-            if t_in.is_cuda:
-                t_in.record_stream(s0)
-        if out is not None and out.is_cuda:
-            out.record_stream(self.streams[4])
+        frame = (reference_image, reference_pose, measurement_images, measurement_poses, full_K)
+        _after_caller(s0, self.streams[4], self.device, frame, out)
         with torch.cuda.stream(s0):
             if self._fill == 0:
                 s0.wait_event(grp["rec_done"])           # every stage of this group's previous use has finished reading its buffers
-            ks["ref_image"].copy_(reference_image, non_blocking=True)
-            ks["ref_pose"].copy_(reference_pose, non_blocking=True)
-            ks["full_K"].copy_(full_K, non_blocking=True)
-            for dst, src in zip(ks["meas_images"], measurement_images):
-                dst.copy_(src, non_blocking=True)
-            for dst, src in zip(ks["meas_poses"], measurement_poses):
-                dst.copy_(src, non_blocking=True)
+            _upload(self.kslots[ki], frame)
         self._pending.append((ki, self._has_state, out))
         self._has_state = True
         self._kslot_of[self.t] = ki
@@ -839,14 +772,13 @@ class LookaheadFusionnet:
             return
         grp = self.groups[self._gi % self.G]
         s0, s1, s2, s3, s4 = self.streams
-        depth_args = (self.min_depth, self.max_depth, self.D)
 
         def run(i, stream, fn, key, after):
             with torch.cuda.stream(stream):
                 if after is not None:
                     stream.wait_event(after)
                 if grp["graph"][i] is None:
-                    grp["graph"][i], grp[key], self._kernels[i] = self._graph_of(fn, stream)
+                    grp["graph"][i], grp[key], self._kernels[i] = self._capture(fn, stream)
                 grp["graph"][i].replay()
                 grp["done"][i].record(stream)
 
@@ -856,14 +788,14 @@ class LookaheadFusionnet:
 
         run(0, s0, head_fn, "head", None)
         run(1, s1, lambda: self.mods["fpn"](*self.mods["fe"].forward_tail(grp["head"])), "pyramid", grp["done"][0])
-        run(2, s2, lambda: _sweep_from_pyramid(grp, grp["pyramid"], 0, *depth_args), "swept", grp["done"][1])
+        run(2, s2, lambda: _sweep_from_pyramid(grp, grp["pyramid"], 0, *self.depth_args), "swept", grp["done"][1])
         run(3, s3, lambda: _stage_enc(self.mods, grp, grp["swept"]), "enc", grp["done"][2])
         for ki, with_state, out in self._pending:
             ks = self.kslots[ki]
             with torch.cuda.stream(s4):
                 s4.wait_event(grp["done"][3])
                 if with_state not in ks["graph"]:
-                    ks["graph"][with_state], _, self._kernels[4] = self._graph_of(self._rec_fn(ks, grp, with_state), s4, rec=True)
+                    ks["graph"][with_state], _, self._kernels[4] = self._capture(lambda: self._run_rec(ks, grp, with_state), s4, ks)
                 ks["graph"][with_state].replay()
                 if out is not None:
                     out.copy_(ks["depth"], non_blocking=True)

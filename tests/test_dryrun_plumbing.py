@@ -101,6 +101,14 @@ for backend in ("fp32", "tc"):
                     "ref_cl": grp["ref_cl"][j:j + 1], "lstm_K": grp["lstm_K"][j:j + 1], "input_gates": grp["input_gates"][j:j + 1]}
             pred, st = pipeline._stage_rec(mods, st, view, sl, half_K[j:j + 1])
             assert tuple(pred.shape) == (1, H, W)
+# pairnet: no ConvLSTM, the decoder reads the encoder's bottom and no recurrent state is carried
+shapes = oracle.state_dict_shapes(D, with_lstm=False)
+w = {t: {k: torch.from_numpy(v) for k, v in synth.make_state_dict(shapes[t], seed=1).items()} for t in shapes}
+mods = pipeline.build_modules(w, device="cpu", n_depth_levels=D, pairnet=True)
+pred, st = pipeline.keyframe(mods, pipeline.KeyframeState(), T(clip["images"][ref_i])[None], T(clip["poses"][ref_i])[None],
+                             [T(clip["images"][j])[None] for j in meas_i], [T(clip["poses"][j])[None] for j in meas_i],
+                             T(clip["K"])[None], n_depth_levels=D)
+assert tuple(pred.shape) == (1, H, W) and st.lstm_state is None
 print("dryrun ok")
 """
 

@@ -100,14 +100,13 @@ def main():
                 return q0.elapsed_time(q1) * 1e3 / reps
 
             # each stage's graph replayed alone: the batched stages once per group of `lookahead` keyframes, the recurrent
-            # stage once per keyframe (its replays advance the static recurrent state, restored afterwards as _graph_of does)
+            # stage once per keyframe (its replays advance the static recurrent state, restored afterwards)
             grp = la.groups[0]
             batched = [alone(grp["graph"][i], la.streams[i], max(a.reps, 50)) for i in range(4)]
-            saved = [t.clone() for t in la._static_state]
+            saved = la._static_state.snapshot()
             ks = next(k for k in la.kslots if True in k["graph"])
             rec_us = alone(ks["graph"][True], la.streams[4], max(a.reps, 200))
-            for dst, src in zip(la._static_state, saved):
-                dst.copy_(src)
+            la._static_state.restore(saved)
             torch.cuda.synchronize()
         print(json.dumps({"engine": "LookaheadFusionnet", "lookahead": a.lookahead, "groups": a.groups, "clips": a.clips,
                           "period_us_per_keyframe_batch": period, "keyframes_per_s": a.clips * 1e6 / period, "host_enqueue_us_per_submit": host_us,
