@@ -175,3 +175,13 @@ def lstm_reference(g, c):
     b_h = so * (b_cn + EPS_LSTM * (cn.abs() + 1)) + EPS_LSTM * 4 * (hn.abs() + so)
     shape = (B, h, w, C)
     return hn.reshape(shape), cn.reshape(shape), b_h.reshape(shape), b_cn.reshape(shape)
+
+
+def check_live(what, *tensors):
+    """operands replayed from an engine's buffers are finite and not all zero: a replay on a zero hidden state or on a buffer
+    nothing wrote proves nothing"""
+    for i, t in enumerate(tensors):
+        if t is None:
+            continue
+        assert bool(torch.isfinite(t).all()), "%s: operand %d is not finite" % (what, i)
+        assert bool((t != 0).any()), "%s: operand %d is all zero" % (what, i)

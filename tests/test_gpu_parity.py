@@ -794,43 +794,60 @@ def test_lookahead_engine_matches_eager_keyframe(oracle, synth, backend, terms, 
         ops.set_conv_backend(old, terms=3)
 
 
-@pytest.mark.parametrize("backend,terms", [("tc", 1), ("tc", 3)])
-def test_engines_match_eager_keyframe_on_the_tensor_core_backend(oracle, synth, backend, terms):
+@pytest.mark.parametrize("backend,terms,point", [
+    pytest.param("tc", 1, None, id="tc-1"), pytest.param("tc", 3, None, id="tc-3"),
+    pytest.param("tc", 1, "pipelined5_b8_256x256", id="tc-1-pipelined5_b8_256x256"),
+    pytest.param("tc", 1, "graphed_b1_256x256", id="tc-1-graphed_b1_256x256")])
+def test_engines_match_eager_keyframe_on_the_tensor_core_backend(oracle, synth, backend, terms, point):
     """GraphedFusionnet and PipelinedFusionnet (2..5 stages, multi-stream, per-stream split-K scratch, PDL, operand planes
     crossing stage boundaries) against eager keyframe() on the SAME backend, different inputs every keyframe: the kernels are
-    deterministic, so the engines must reproduce the eager results bit for bit."""
+    deterministic, so the engines must reproduce the eager results bit for bit.  At 64x96, B = 1, every engine; at bench.py's
+    256x256, the 5-stage engine of its batched_8 point (a distinct clip in each of the 8 rows) and the graphed engine of its
+    sequential-latency point: there the engines run eager's kernels with eager's split decisions at bench.py's sizes, so
+    cross-stream buffer reuse or aliased split-K scratch would show."""
     from dvmvs import _ops as ops
     from dvmvs import pipeline
-    H, W, D, M = 64, 96, 64, 2
+    H, W, D, M = (64, 96, 64, 2) if point is None else (256, 256, 64, 2)
+    B = 8 if point == "pipelined5_b8_256x256" else 1
     w = helpers.oracle_weights(oracle, synth, 11, n_depth_levels=D)
     old = ops.conv_backend()
     ops.set_conv_backend(backend, terms=terms, stride2=True)
     try:
         mods = helpers.build_product_modules(w, n_depth_levels=D)
-        clip = synth.make_clip(5, 7, H, W, M)
-        K = _cuda(clip["K"])[None]
+        clips = [synth.make_clip(5 + c, 7 if point is None else 6, H, W, M) for c in range(B)]
+        K = torch.from_numpy(np.stack([c["K"] for c in clips])).to(DEV)
         st = pipeline.KeyframeState()
-        eng = pipeline.GraphedFusionnet(mods, batch=1, height=H, width=W, n_measurement_frames=M, n_depth_levels=D)
-        pipes = [pipeline.PipelinedFusionnet(mods, batch=1, height=H, width=W, n_measurement_frames=M, n_depth_levels=D, n_stages=ns)
-                 for ns in (2, 3, 5)]
+        kw = dict(batch=B, height=H, width=W, n_measurement_frames=M, n_depth_levels=D)
+        eng = pipeline.GraphedFusionnet(mods, **kw) if point != "pipelined5_b8_256x256" else None
+        stages = (2, 3, 5) if point is None else ((5,) if point == "pipelined5_b8_256x256" else ())
+        pipes = [pipeline.PipelinedFusionnet(mods, n_stages=ns, **kw) for ns in stages]
         expected, graphed, piped = [], [], [[] for _ in pipes]
+        stack = lambda pick: torch.from_numpy(np.stack([pick(c) for c in clips])).to(DEV)
         with torch.no_grad():
-            for ref_i, meas_i in clip["frames"]:
-                args = (_cuda(clip["images"][ref_i])[None], _cuda(clip["poses"][ref_i])[None], [_cuda(clip["images"][j])[None] for j in meas_i],
-                        [_cuda(clip["poses"][j])[None] for j in meas_i], K)
+            for t in range(len(clips[0]["frames"])):
+                ref_i = lambda c: c["frames"][t][0]
+                meas_i = lambda c, m: c["frames"][t][1][m]
+                args = (stack(lambda c: c["images"][ref_i(c)]), stack(lambda c: c["poses"][ref_i(c)]),
+                        [stack(lambda c: c["images"][meas_i(c, m)]) for m in range(M)],
+                        [stack(lambda c: c["poses"][meas_i(c, m)]) for m in range(M)], K)
                 a, st = pipeline.keyframe(mods, st, *args, n_depth_levels=D)
                 expected.append(a.clone())
-                graphed.append(eng.step(*args).clone())
+                if eng is not None:
+                    graphed.append(eng.step(*args).clone())
                 for pi, pipe in enumerate(pipes):
-                    out = torch.empty((1, H, W), dtype=torch.float32, device=DEV)
+                    out = torch.empty((B, H, W), dtype=torch.float32, device=DEV)
                     pipe.submit(*args, out=out)
                     piped[pi].append(out)
             for pipe in pipes:
                 pipe.synchronize()
+        assert B == 1 or not torch.equal(expected[-1][0], expected[-1][-1]), "the batch rows hold the same clip"
+        print("engines vs eager keyframe (%s, %d terms, %s): %d keyframes, B=%d, graphed %s, pipelined %s" % (
+            backend, terms, point or "64x96", len(expected), B, eng is not None, stages))
         for t, e in enumerate(expected):
-            assert torch.equal(graphed[t], e), "graph engine, keyframe %d: max diff %.3e" % (t, float((graphed[t] - e).abs().max()))
+            if eng is not None:
+                assert torch.equal(graphed[t], e), "graph engine, keyframe %d: max diff %.3e" % (t, float((graphed[t] - e).abs().max()))
             for pi in range(len(pipes)):
-                assert torch.equal(piped[pi][t], e), "pipeline %d, keyframe %d: max diff %.3e" % (pi, t, float((piped[pi][t] - e).abs().max()))
+                assert torch.equal(piped[pi][t], e), "pipeline %d, keyframe %d: max diff %.3e" % (stages[pi], t, float((piped[pi][t] - e).abs().max()))
     finally:
         ops.set_conv_backend(old, terms=3)
 

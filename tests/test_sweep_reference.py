@@ -84,14 +84,22 @@ CASES = {
     "forward_motion": (1, 64, 96, 64, 2),
     "identity": (1, 32, 48, 16, 1),
     "magnitudes": (1, 64, 64, 32, 2),
+    # bench.py's roofline launches (time_sweep): nb clips at 128x128, D = 64, M = 2, features randn x 4 seeded with nb, clip 0's
+    # keyframe-0 poses repeated over the batch
+    "roofline_1": (1, 128, 128, 64, 2),
+    "roofline_8": (8, 128, 128, 64, 2),
+    "roofline_32": (32, 128, 128, 64, 2),
 }
 
 
 def make_case(name):
     """geometry (fp32, CPU) and seeded features (scale 4 unless the case says otherwise) of one case"""
     B, h, w, D, M = CASES[name]
-    seed = sum(map(ord, name))
-    if name == "benchmark_group":
+    seed = B if name.startswith("roofline_") else sum(map(ord, name))
+    if name.startswith("roofline_"):
+        pose1, pose2s, K = _clip_geometry(1, 2 * h, 2 * w, M)
+        pose1, pose2s, K = pose1.repeat(B, 1, 1), [p.repeat(B, 1, 1) for p in pose2s], K.repeat(B, 1, 1)
+    elif name == "benchmark_group":
         pose1, pose2s, K = _clip_geometry(4, 2 * h, 2 * w, M)
     elif name == "c3":
         pose1, pose2s, K = _clip_geometry(1, 2 * h, 2 * w, M)
@@ -198,6 +206,8 @@ def _assert_reach(c):
     G, Kt, _, _ = R.frame_geometry(c["pose1"], c["pose2s"][0], c["K"])
     if name == "benchmark_group":
         assert B * ((w + 15) // 16) * ((h + 3) // 4) >= 6 * 132, "fewer than ~8 tiles per persistent CTA"
+    if name.startswith("roofline_"):
+        assert (h, w, D, M) == (128, 128, 64, 2) and bool((c["pose1"] == c["pose1"][:1]).all())
     if name == "partial_tiles":
         assert h % 4 and w % 16 and M & (M - 1) and B > 1
     if name == "tiny":
@@ -251,11 +261,25 @@ def _check_all(c, outs, refs, tag=""):
     return rows
 
 
+def on_rows(c, outs, planes1, planes2):
+    """the case, the kernels' outputs and operands restricted to the batch rows tools.engine_record.batch_rows picks: the sweep
+    computes every output row from its own operand row, so the reference over these rows is exact for them"""
+    from tools.engine_record import batch_rows
+    rows = batch_rows(c["B"])
+    if len(rows) == c["B"]:
+        return c, outs, planes1, planes2
+    r = torch.tensor(rows)
+    c = dict(c, B=len(rows), pose1=c["pose1"][r], pose2s=[p[r] for p in c["pose2s"]], K=c["K"][r], f1=c["f1"][r], f2s=[f[r] for f in c["f2s"]])
+    r = r.to(DEV)
+    return c, {k: v.index_select(0, r) for k, v in outs.items()}, planes1.index_select(1, r), [p.index_select(1, r) for p in planes2]
+
+
 @pytest.mark.parametrize("name", list(CASES))
 def test_sweep_kernels_vs_fp64_reference(name, ops):
     c = make_case(name)
     _assert_reach(c)
     outs, planes1, planes2 = run_kernels(c, ops)
+    c, outs, planes1, planes2 = on_rows(c, outs, planes1, planes2)
     refs = references(c, planes1, planes2)
     if name == "magnitudes":
         r = (planes1[0].float() * 2.0 ** -5).half()
@@ -302,27 +326,55 @@ def test_sweep_tc_band_capacity_vs_fp64_reference(qcap, ops, tmp_path):
 
 
 def test_sweep_of_the_benchmarked_engine_vs_fp64_reference(ops):
-    """the plane_sweep_tc launch of bench.py's default engine (LookaheadFusionnet, 1-term operands, bench.py's input size), recorded
-    while it primes and replayed on its own buffers: the FPN features it really sweeps, under the 1-term bound"""
+    """the sweep of every operating point bench.py reports (tools/engine_record.py POINTS), each checked by _engine_sweep_at; every
+    point that fails is reported"""
     sys.path.insert(0, REPO_DIR)
-    from tools.engine_record import engine_calls
-    _, calls = engine_calls(("plane_sweep_tc",))
+    from tools.engine_record import POINTS
+    failed = {}
+    for point in POINTS:
+        try:
+            _engine_sweep_at(ops, point)
+        except AssertionError as e:
+            failed[point] = str(e)
+        torch.cuda.empty_cache()
+    assert not failed, "\n".join("%s: %s" % kv for kv in failed.items())
+
+
+def _engine_sweep_at(ops, point):
+    """the plane_sweep_tc launch of the engine bench.py runs at this operating point, recorded while it runs as bench.py runs it
+    and replayed on its own buffers: the FPN features it really sweeps, under the bound of the point's terms, on the batch rows
+    tools.engine_record.batch_rows picks.  Checks the sweep's batch, D, M and terms against the point's configuration."""
+    import time
+    from tools.engine_record import batch_rows, engine_calls, point_config
+    t0 = time.perf_counter()
+    cfg = point_config(point)
+    _, calls = engine_calls(("plane_sweep_tc",), point=point)
     sweeps = [v for k, v in calls.items() if k[0] == "plane_sweep_tc"]
-    assert sweeps, "the engine launched no plane_sweep_tc"
+    assert len(sweeps) == 1, "%s: the engine launched %d plane_sweep_tc call sites" % (point, len(sweeps))
     for args, kw, _, _ in sweeps:
         ref_pair, meas_pairs, pose1, pose2s, K, mn, mx, D = args[:8]
         terms = kw.get("terms", 3)
+        B, h, w, _ = ref_pair[0].shape
+        expect_B = cfg["batch"] * (cfg["lookahead"] if cfg["engine"] == "lookahead" else 1)
+        assert (B, D, len(pose2s), terms) == (expect_B, cfg["n_depth_levels"], cfg["n_measurement_frames"], cfg["terms"]), (
+            "%s: sweep B, D, M, terms = %s, expected %s" % (point, (B, D, len(pose2s), terms),
+                                                          (expect_B, cfg["n_depth_levels"], cfg["n_measurement_frames"], cfg["terms"])))
+        rows = torch.tensor(batch_rows(B), device=DEV)
+        sel = lambda t: t.index_select(0, rows)
+        pl = lambda p: (sel(p[0]), sel(p[1]) if terms == 3 else None)
+        from tests.tc_reference import check_live
+        check_live("%s sweep" % point, sel(ref_pair[0]), *[sel(p[0]) for p in meas_pairs])
         got = ops.plane_sweep_tc(ref_pair, meas_pairs, pose1, pose2s, K, mn, mx, D, terms=terms)
         torch.cuda.synchronize()
-        pl = lambda p: (p[0], p[1] if terms == 3 else None)
-        ref = R.sweep_reference("tc%d" % terms, pose1.float(), [p.float() for p in pose2s], K.float(), mn, mx, D,
+        ref = R.sweep_reference("tc%d" % terms, sel(pose1).float(), [sel(p).float() for p in pose2s], sel(K).float(), mn, mx, D,
                                 planes1=pl(ref_pair), planes2=[pl(p) for p in meas_pairs])
-        B, h, w, _ = ref_pair[0].shape
-        c = dict(name="engine", B=B, h=h, w=w, D=D, M=len(pose2s), pose1=pose1.cpu(), pose2s=[p.cpu() for p in pose2s], K=K.cpu())
-        worst, acc, tight = R.check_sweep("engine sweep B=%d %dx%d terms=%d" % (B, h, w, terms), got, ref, _describe(c))
+        c = dict(name="engine", B=len(rows), h=h, w=w, D=D, M=len(pose2s), pose1=sel(pose1).cpu(), pose2s=[sel(p).cpu() for p in pose2s],
+                 K=sel(K).cpu())
+        worst, acc, tight = R.check_sweep("%s sweep B=%d %dx%d terms=%d" % (point, B, h, w, terms), sel(got), ref, _describe(c))
         feat = max(float(ref_pair[0].float().abs().max()), max(float(p[0].float().abs().max()) for p in meas_pairs))
-        print("engine sweep B=%d %dx%d D=%d M=%d terms=%d: err/bound %.3f  err/(u n S) %.3f  ill-conditioned %d  median bound/sum w|s| "
-              "%.2e; largest |feature| %.4g, largest |S| %.4g (fp16 max %g)" % (B, h, w, D, len(pose2s), terms, worst, acc, ref.n_ill,
-                                                                               tight, feat, ref.smax, FP16_MAX))
+        print("%s sweep B=%d (rows %s) %dx%d D=%d M=%d terms=%d: err/bound %.3f  err/(u n S) %.3f  ill-conditioned %d  median bound/sum "
+              "w|s| %.2e; largest |feature| %.4g, largest |S| %.4g (fp16 max %g); %.1f s" % (
+                  point, B, batch_rows(B), h, w, D, len(pose2s), terms, worst, acc, ref.n_ill, tight, feat, ref.smax, FP16_MAX,
+                  time.perf_counter() - t0))
         assert acc <= C_ACC / 8
         assert ref.smax < FP16_MAX / 8, "the engine's correlations come within 8x of the fp16 range of the 1-term S"

@@ -51,7 +51,7 @@ def _fill_lo(ptr, n):
 
 class NativeSpy:
     """Wraps the library's dvmvs_conv2d_tc / dvmvs_conv2d_halo while active: records the split count (dvmvs_conv2d_tc_ksplit on
-    the same descriptor) and the output tile of every conv2d_tc launch, and fills the lo plane of every fp16 output of a
+    the same descriptor), the output tile, block_n, terms and batch of every conv2d_tc launch, and fills the lo plane of every fp16 output of a
     hi-plane-only launch with SENTINEL first, so that a test can tell the plane was left alone."""
 
     def __enter__(self):
@@ -64,7 +64,8 @@ class NativeSpy:
             d = dref._obj
             pad = (d.ksize - 1) // 2
             Ho, Wo = (d.Hin + 2 * pad - d.ksize) // d.stride + 1, (d.Win + 2 * pad - d.ksize) // d.stride + 1
-            self.tc.append({"ksplit": int(L.dvmvs_conv2d_tc_ksplit(dref)), "tile": "8x16" if (Wo <= 8 and Ho > 8) else "16x8"})
+            self.tc.append({"ksplit": int(L.dvmvs_conv2d_tc_ksplit(dref)), "tile": "8x16" if (Wo <= 8 and Ho > 8) else "16x8",
+                            "block_n": int(d.block_n), "terms": int(d.terms), "B": int(d.B)})
             if d.out_hi_only:
                 n = d.B * Ho * Wo * d.Cout
                 _fill_lo(d.out_planes, n)
@@ -346,9 +347,9 @@ def test_lstm_deferred_gate_gemm_and_epilogue(ops, terms):
 
 
 # ------------------------------------------------------------------------------------------------ every layer the benchmark runs
-def _real_channels(planes_list, src_channels, blocked, packed):
-    """hi planes of the operands -> (B, Cin, H, W) of the real channels in the weights' order"""
-    hi = [_blk_to_nchw(t[0]) if blocked else _nchw(t[0]) for t in planes_list]
+def _real_channels(planes_list, src_channels, blocked, packed, plane=0):
+    """hi (plane 0) or lo (plane 1) planes of the operands -> (B, Cin, H, W) of the real channels in the weights' order"""
+    hi = [_blk_to_nchw(t[plane]) if blocked else _nchw(t[plane]) for t in planes_list]
     if packed:        # one operand tensor holding every source (at 8-channel boundaries on the blocked path, back to back otherwise)
         out, off = [], 0
         for cr in src_channels:
@@ -358,26 +359,42 @@ def _real_channels(planes_list, src_channels, blocked, packed):
     return torch.cat([t[:, :cr] for t, cr in zip(hi, src_channels)], 1).double()
 
 
-def _replay_tc(args, kw, lay, spy):
+def _at(t, rows, dim=0):
+    return None if t is None else t.index_select(dim, rows)
+
+
+def _operands(planes_list, src_channels, blocked, packed, terms, rows):
+    """(hi, lo) operands of the batch rows `rows` in fp64; lo is None for 1-term products (its plane is not written then)"""
+    hi = _at(_real_channels(planes_list, src_channels, blocked, packed), rows)
+    lo = _at(_real_channels(planes_list, src_channels, blocked, packed, 1), rows) if terms == 3 else None
+    R.check_live("operands", hi)
+    return hi, lo
+
+
+def _replay_tc(args, kw, lay, spy, rows):
     from dvmvs import _ops as ops
     planes, ptc = args[0], args[1]
-    x = _real_channels(planes, [ptc.cin] if lay.pack_sources else lay.src_channels, False, lay.pack_sources)
+    terms = kw.get("terms", 3)
+    x, xl = _operands(planes, [ptc.cin] if lay.pack_sources else lay.src_channels, False, lay.pack_sources, terms, rows)
     with torch.no_grad():
         r = ops.conv2d_tc(*args, **kw)
         torch.cuda.synchronize()
     ks = spy.tc[-1]["ksplit"]
     res = kw.get("residual")
-    ref = R.conv_reference(x, None, lay.pc.weight, kw.get("terms", 3), ptc.stride, ptc.bias, None if res is None else _nchw(res),
+    ref = R.conv_reference(x, xl, lay.pc.weight, terms, ptc.stride, ptc.bias, None if res is None else _nchw(_at(res, rows)),
                            kw.get("residual_mode", R.RES_NONE), ptc.act, kw.get("aux"), k_padded=ptc.ktot, ksplit=ks)
-    w, a = _check_outputs("", ref, f32=r[0], planes=r[1], blk=kw.get("blk_out"), aux=r[2] if kw.get("aux") else None, hi_only=True)
-    return ks, spy.tc[-1]["tile"], w, a
+    w, a = _check_outputs("", ref, f32=_at(r[0], rows), planes=_at(r[1], rows, 1), blk=_at(kw.get("blk_out"), rows, 1),
+                          aux=_at(r[2], rows) if kw.get("aux") else None, hi_only=terms == 1)
+    return spy.tc[-1], w, a
 
 
-def _replay_deferred(args, kw, lay, gates_call, spy):
+def _replay_deferred(args, kw, lay, gates_call, spy, rows):
     from dvmvs import _ops as ops
     planes, ptc = args[0], args[1]
-    x = _real_channels(planes, lay.src_channels, False, False)
+    terms = kw.get("terms", 3)
+    x, xl = _operands(planes, lay.src_channels, False, False, terms, rows)
     (_, c), gkw = gates_call[0], gates_call[1]
+    R.check_live("deferred gate epilogue", _at(c, rows), _at(gkw.get("addend"), rows))
     with torch.no_grad():
         r = ops.conv2d_tc(*args, **kw)
         ws, offset, n_parts, stride = r[1]
@@ -388,94 +405,168 @@ def _replay_deferred(args, kw, lay, gates_call, spy):
             g = g + ws[offset // 4 + sp * stride:offset // 4 + sp * stride + total]
         h_out, c_out = ops.lstm_gates(None, c, parts=r[1], addend=gkw.get("addend"))
         torch.cuda.synchronize()
-    ref = R.conv_reference(x, None, lay.pc.weight, kw.get("terms", 3), k_padded=ptc.ktot, ksplit=n_parts)
-    wg, acc = _check_outputs("", ref, f32=g.view(B, h, w, 4 * C))
+    ref = R.conv_reference(x, xl, lay.pc.weight, terms, k_padded=ptc.ktot, ksplit=n_parts)
     g = g.view(B, h, w, 4 * C)
+    wg, acc = _check_outputs("", ref, f32=_at(g, rows))
     if gkw.get("addend") is not None:
         g = g + gkw["addend"]
-    we = _check_lstm("gate epilogue", g, c, h_out, c_out)
-    return n_parts, spy.tc[-1]["tile"], max(wg, we), acc
+    we = _check_lstm("gate epilogue", _at(g, rows), _at(c, rows), _at(h_out, rows), _at(c_out, rows))
+    return dict(spy.tc[-1], gates=_lstm_instantiation(B, C, h * w)), max(wg, we), acc
 
 
-def _replay_halo(args, kw, lay):
+def _replay_gates(args, rows):
+    """the plain gate epilogue (the gate convolution did not split, so it ran with its own finishing pass and the state-
+    independent half as its residual): lstm_gates on the pre-activations the engine handed it"""
+    from dvmvs import _ops as ops
+    g, c = args
+    R.check_live("lstm_gates", _at(g, rows), _at(c, rows))
+    with torch.no_grad():
+        h_out, c_out = ops.lstm_gates(g, c)
+        torch.cuda.synchronize()
+    B, h, w, C = c.shape
+    return _lstm_instantiation(B, C, h * w), _check_lstm("gate epilogue", _at(g, rows), _at(c, rows), _at(h_out, rows), _at(c_out, rows))
+
+
+def _replay_halo(args, kw, lay, rows):
     from dvmvs import _ops as ops
     blks, ph = args[0], args[1]
+    terms = kw.get("terms", 3)
+    x, xl = _operands(blks, lay.src_channels, True, lay.pack_sources, terms, rows)
     with torch.no_grad():
         f32, oblk, onhwc = ops.conv2d_halo(*args, **kw)
         torch.cuda.synchronize()
-    x = _real_channels(blks, lay.src_channels, True, lay.pack_sources)
     res = kw.get("residual")
-    ref = R.conv_reference(x, None, lay.pc.weight, kw.get("terms", 3), 1, ph.bias, None if res is None else _nchw(res),
+    ref = R.conv_reference(x, xl, lay.pc.weight, terms, 1, ph.bias, None if res is None else _nchw(_at(res, rows)),
                            R.RES_NONE if res is None else R.RES_SAME, ph.act, k_padded=ph.ksize ** 2 * ph.n_groups * ph.kc)
-    return _check_outputs("", ref, f32=f32, planes=onhwc, blk=oblk, hi_only=True)
+    return _check_outputs("", ref, f32=_at(f32, rows), planes=_at(onhwc, rows, 1), blk=_at(oblk, rows, 1), hi_only=terms == 1)
 
 
-def _replay_expand(args, kw):
+def _replay_expand(args, kw, rows):
     from dvmvs import _ops as ops
     act, expand, dw = args[0], args[1], args[2]
     terms = kw.get("terms", args[3] if len(args) > 3 else None)
+    terms = ops._TC_TERMS if terms is None else terms               # None: the terms of the call's family, as the engine ran it
+    pc = expand.pc
+    x, xl = (_at(_nchw(p)[:, :pc.cin].double(), rows) for p in act.get_planes())
+    R.check_live("expand_dwconv", x)
     with torch.no_grad():
         out = ops.expand_dwconv(*args, **kw)
         torch.cuda.synchronize()
-    pc = expand.pc
-    x = _nchw(act.get_planes()[0])[:, :pc.cin].double()
-    e = R.conv_reference(x, None, pc.weight, 1 if terms is None else terms, 1, pc.bias, act=pc.act, k_padded=expand._ptc.ktot)
+    e = R.conv_reference(x, xl, pc.weight, terms, 1, pc.bias, act=pc.act, k_padded=expand._ptc.ktot)
     k = dw.ksize
     wd = dw.weight.permute(2, 0, 1).unsqueeze(1).double()             # [k][k][C] -> (C,1,k,k)
     y = F.conv2d(e.y, wd, dw.bias.double(), dw.stride, k // 2, groups=dw.channels)
     b = F.conv2d(e.bound, wd.abs(), None, dw.stride, k // 2, groups=dw.channels)
     b = b + (k * k + 2) * R.U * (F.conv2d(e.y.abs(), wd.abs(), None, dw.stride, k // 2, groups=dw.channels) + dw.bias.double().abs().view(1, -1, 1, 1))
     y, b = R.activation(y, b, dw.act)
-    rows = []
-    R.check("expand_dwconv", _nchw(out[0]).float(), y, R.fp16_bound(y, b), report=rows)
-    return rows[0][1], e.eps_acc
+    rows_ = []
+    R.check("expand_dwconv", _nchw(_at(out[0], rows)).float(), y, R.fp16_bound(y, b), report=rows_)
+    return rows_[0][1], e.eps_acc, terms
 
 
-@pytest.mark.parametrize("height,width", [(256, 320), (320, 256)])
-def test_every_benchmark_layer_vs_fp64_reference(ops, height, width):
-    """Records every conv2d_tc, conv2d_halo, expand_dwconv and deferred gate call of bench.py's engine (seed-7 weights, 1-term
-    operands) while it primes at this input size, and replays each on its recorded operands against the fp64 reference.  One
-    line per layer; a failure names the layer."""
-    from tools.engine_record import engine_calls, layer_names
-    mods, calls = engine_calls(("conv2d_tc", "conv2d_halo", "expand_dwconv", "lstm_gates"), height=height, width=width)
+def _point_params():
+    """bench.py's operating points (tools/engine_record.py POINTS) at their own input sizes, and the headline engine at 256x320
+    and 320x256: the portrait size is the only one whose 10x8 bottleneck runs the 8-wide tile"""
+    from tools.engine_record import POINTS
+    return ([pytest.param("value", 256, 320, id="256-320"), pytest.param("value", 320, 256, id="320-256")] +
+            [pytest.param(p, None, None, id=p) for p in POINTS])
+
+
+@pytest.mark.parametrize("point,height,width", _point_params())
+def test_every_benchmark_layer_vs_fp64_reference(ops, point, height, width):
+    """Records every conv2d_tc, conv2d_halo, expand_dwconv and ConvLSTM gate call (deferred pair or plain epilogue) of the engine
+    bench.py runs at this operating point (seed-7 weights, the point's operand terms and batch, clip b in batch row b), and replays
+    each on its recorded operands against the fp64 reference, on the batch rows tools.engine_record.batch_rows picks.  One line
+    per layer; a failure names the layer.  Then checks the facts that make the point differ from the headline (batch, split
+    counts, block_n, gate path and instantiation, terms, aggregator0's cost-volume channels)."""
+    import time
+    from tools.engine_record import batch_rows, engine_calls, layer_names, point_config, trunk_batch
+    t0 = time.perf_counter()
+    cfg = point_config(point, height, width)
+    mods, calls = engine_calls(("conv2d_tc", "conv2d_halo", "expand_dwconv", "lstm_gates"), point=point, height=height, width=width)
     names = layer_names(mods)
+    gate_layer = mods["lstm"].lstm_cell.packed()[1]             # conv(W[:, Cin:], h): the gate convolution on the recurrent state
+    agg0 = mods["cve"].packed()[0]
     gates_calls = [v for k, v in calls.items() if k[0] == "lstm_gates" and k[2]]
-    seen = {"conv2d_tc": 0, "conv2d_halo": 0, "expand_dwconv": 0, "deferred": 0}
+    seen = {"conv2d_tc": 0, "conv2d_halo": 0, "expand_dwconv": 0, "deferred": 0, "lstm_gates": 0}
     tiles, worst_all, acc_all = set(), 0.0, 0.0
+    trunk, terms_seen, tc_launches, gate, agg0_seen = set(), set(), [], {}, False
     print()
     for key, (args, kw, lay, on_rec) in calls.items():
         kind = key[0]
-        if kind == "lstm_gates":
-            continue
-        layer = names.get(id(lay if lay is not None else args[1]), "?")
+        if kind == "lstm_gates" and key[2]:
+            continue                    # replayed with its gate GEMM
+        layer = names.get(id(lay if lay is not None else args[1]), "?") if kind != "lstm_gates" else "lstm gates"
         if kind == "conv2d_halo":
             path, shape = "halo", (args[0][0].shape[1],) + tuple(args[0][0].shape[3:5])
         elif kind == "conv2d_tc":
             path, shape = "tc deferred+gates" if kw.get("defer_finish") else "tc", tuple(args[0][0].shape[1:4])
+        elif kind == "lstm_gates":
+            path, shape = "gates", tuple(args[1].shape[:3])
         else:
             path, shape = "expand_dw", tuple(args[0].get_planes().shape[1:4])
-        ks, tile, acc = 1, "-", 0.0
+        rows = torch.tensor(batch_rows(shape[0]), device=DEV)
+        launch, acc, extra = {}, 0.0, ""
         try:
             with NativeSpy() as spy:
                 if path == "tc deferred+gates":
                     assert len(gates_calls) == 1, "expected one deferred gate epilogue, recorded %d" % len(gates_calls)
-                    ks, tile, worst, acc = _replay_deferred(args, kw, lay, gates_calls[0], spy)
-                    assert ks > 1
+                    launch, worst, acc = _replay_deferred(args, kw, lay, gates_calls[0], spy, rows)
+                    assert launch["ksplit"] > 1
                     seen["deferred"] += 1
+                    extra = " gates=<%d,%d>" % launch["gates"]
                 elif path == "tc":
-                    ks, tile, worst, acc = _replay_tc(args, kw, lay, spy)
+                    launch, worst, acc = _replay_tc(args, kw, lay, spy, rows)
+                elif path == "gates":
+                    inst, worst = _replay_gates(args, rows)
+                    gate["plain"] = inst
+                    extra = " gates=<%d,%d>" % inst
                 elif path == "halo":
-                    worst, acc = _replay_halo(args, kw, lay)
+                    worst, acc = _replay_halo(args, kw, lay, rows)
                 else:
-                    worst, _ = _replay_expand(args, kw)
+                    worst, _, expand_terms = _replay_expand(args, kw, rows)
         except AssertionError as e:
-            raise AssertionError("layer %s (%s%s, input B,H,W=%s): %s" % (layer, path, ", recurrent stage" if on_rec else "", shape, e)) from None
+            raise AssertionError("%s: layer %s (%s%s, input B,H,W=%s): %s" % (point, layer, path, ", recurrent stage" if on_rec else "", shape, e)) from None
         seen[kind] += 1
         if path.startswith("tc"):
-            tiles.add(tile)
+            tiles.add(launch["tile"])
+            tc_launches.append((layer, launch))
+            terms_seen.add(launch["terms"])
+            if lay is gate_layer:
+                gate["conv"] = launch
+        elif path == "halo":
+            terms_seen.add(kw["terms"])
+        elif path == "expand_dw":
+            terms_seen.add(expand_terms)
+        if layer.startswith("fe"):
+            trunk.add(shape[0])
+        if lay is agg0:
+            agg0_seen = True
+            assert lay.src_channels == [32, cfg["n_depth_levels"]], "%s: aggregator0 reads %s" % (point, lay.src_channels)
         worst_all, acc_all = max(worst_all, worst), max(acc_all, acc)
-        _report("%-34s %-18s B,H,W=%-14s ksplit=%d tile=%-4s err/bound %.3f  err/(u n S) %.3f" % (layer, path, shape, ks, tile, worst, acc))
-    _report("%dx%d: %s; worst err/bound %.3f, worst err/(u n S) %.3f (C_ACC = %g)" % (height, width, seen, worst_all, acc_all, R.C_ACC))
-    assert all(v > 0 for v in seen.values()), seen
-    if (height, width) == (320, 256):
+        facts = ("ksplit=%d block_n=%-3d terms=%d tile=%-4s" % (launch["ksplit"], launch["block_n"], launch["terms"], launch["tile"])
+                 if launch else "%-34s" % "")
+        _report("%-34s %-18s B,H,W=%-15s %s rows=%d err/bound %.3f  err/(u n S) %.3f%s" % (layer, path, shape, facts, len(rows), worst, acc, extra))
+    deferred = seen["deferred"] > 0
+    _report("%s %dx%d B=%d terms=%d: %s; trunk batch %s; gate %s; worst err/bound %.3f, worst err/(u n S) %.3f (C_ACC = %g); %.1f s" % (
+        point, cfg["height"], cfg["width"], cfg["batch"], cfg["terms"], seen, sorted(trunk),
+        "deferred+gates ksplit=%d" % gate["conv"]["ksplit"] if deferred else "plain block_n=%d ksplit=%d <%d,%d>" % (
+            (gate["conv"]["block_n"], gate["conv"]["ksplit"]) + gate["plain"]), worst_all, acc_all, R.C_ACC, time.perf_counter() - t0))
+    # what makes this point this point
+    assert all(seen[k] > 0 for k in ("conv2d_tc", "conv2d_halo", "expand_dwconv")), seen
+    assert "conv" in gate and agg0_seen, "%s: the gate convolution or aggregator0 was not replayed" % point
+    assert trunk == {trunk_batch(cfg)}, "%s: trunk batch %s, expected %d" % (point, sorted(trunk), trunk_batch(cfg))
+    assert terms_seen == {cfg["terms"]}, "%s: tensor-core calls at terms %s, expected %d" % (point, terms_seen, cfg["terms"])
+    assert gate["conv"]["B"] == cfg["batch"]
+    if cfg["batch"] == 1:         # the gate GEMM (Cout 2048 on the 8x8 map) has 16 CTAs: it splits and the epilogue is its finishing pass
+        assert deferred and seen["lstm_gates"] == 0, "%s: no deferred gate GEMM + epilogue pair (%s)" % (point, seen)
+        assert gate["conv"]["block_n"] == 128
+    else:                         # >= 66 CTAs: no split, so no deferred pair; the plain epilogue, wide instantiation
+        assert not deferred and seen["lstm_gates"] == 1, "%s: expected the plain gate epilogue (%s)" % (point, seen)
+        assert gate["conv"]["ksplit"] == 1 and gate["plain"] == (8, 32), (gate["conv"], gate["plain"])
+        assert gate["conv"]["block_n"] == (64 if cfg["batch"] >= 16 else 128), gate["conv"]
+    if cfg["batch"] == 32:
+        split = [(n, l["ksplit"]) for n, l in tc_launches if l["ksplit"] != 1]
+        assert not split, "%s: conv2d_tc calls that split: %s" % (point, split)
+    if (cfg["height"], cfg["width"]) == (320, 256):
         assert "8x16" in tiles, "the 10x8 bottleneck of a portrait input no longer runs the 8-wide tile"
