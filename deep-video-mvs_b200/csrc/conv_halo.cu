@@ -406,6 +406,9 @@ extern "C" int dvmvs_conv2d_halo(const dvmvs_conv_halo_desc* d, dvmvs_stream_t s
   DVMVS_REQUIRE(d->B > 0 && d->H > 0 && d->W > 0 && d->Cout > 0 && d->Cout % 8 == 0 && d->w_hi && (d->terms == 1 || d->w_lo),
                 "conv2d_halo: bad shape / null weights (Cout must be a multiple of 8)");
   DVMVS_REQUIRE(d->out_f32 || d->out_blk || d->out_nhwc, "conv2d_halo: no output");
+  DVMVS_REQUIRE((uintptr_t)d->bias % 16 == 0 && (uintptr_t)d->residual % 16 == 0 && (uintptr_t)d->out_f32 % 16 == 0 &&
+                    (uintptr_t)d->out_blk % 16 == 0 && (uintptr_t)d->out_nhwc % 16 == 0,
+                "conv2d_halo: bias, residual and outputs must be 16-byte aligned (the epilogue moves 8 channels as 16-byte vectors)");
   HaloParams p;
   memset(&p, 0, sizeof(p));
   p.ksize = d->ksize; p.pad = (d->ksize - 1) / 2; p.terms = d->terms; p.kc = d->kc; p.n_src = d->n_src;

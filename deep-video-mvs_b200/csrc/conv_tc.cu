@@ -633,6 +633,11 @@ extern "C" int dvmvs_conv2d_tc(const dvmvs_conv_tc_desc* d, dvmvs_stream_t strea
   p.out_f32 = d->out_f32; p.out_planes = (__half*)d->out_planes; p.aux_out = d->aux_out;
   p.out_blk = (__half*)d->out_blk;
   DVMVS_REQUIRE(!d->out_blk || (d->out_planes && d->Cout % 8 == 0), "conv2d_tc: out_blk needs out_planes and Cout %% 8 == 0");
+  // Cout % 8 == 0: the epilogue (tc_emit8) loads bias / residual and stores every output but aux_out as 16-byte vectors, and the
+  // split-K partial sums go to the workspace as float4
+  DVMVS_REQUIRE(d->Cout % 8 != 0 || ((uintptr_t)d->bias % 16 == 0 && (uintptr_t)d->residual % 16 == 0 && (uintptr_t)d->out_f32 % 16 == 0 &&
+                                     (uintptr_t)d->out_planes % 16 == 0 && (uintptr_t)d->out_blk % 16 == 0 && (uintptr_t)d->workspace % 16 == 0),
+                "conv2d_tc: bias, residual, outputs and workspace must be 16-byte aligned");
   p.aux_mult = d->aux_mult; p.aux_base = d->aux_base; p.act = d->act;
   p.hi_only = d->out_hi_only ? 1 : 0;
   cudaStream_t s = (cudaStream_t)stream;

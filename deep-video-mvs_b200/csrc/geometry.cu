@@ -1003,6 +1003,8 @@ extern "C" int dvmvs_hidden_warp_backward(const float* grad_out, const float* de
                                           dvmvs_stream_t stream) {
   DVMVS_REQUIRE(grad_out && depth && cur_pose && K && grad_h_in, "hidden_warp_backward: null pointer");
   DVMVS_REQUIRE(B > 0 && C > 0 && C % 4 == 0 && h > 1 && w > 1, "hidden_warp_backward: bad shape (C must be a multiple of 4)");
+  // float4 loads of grad_out, red.global.add.v4.f32 into grad_h_in
+  DVMVS_REQUIRE((uintptr_t)grad_out % 16 == 0 && (uintptr_t)grad_h_in % 16 == 0, "hidden_warp_backward: grad_out and grad_h_in must be 16-byte aligned");
   cudaStream_t s = (cudaStream_t)stream;
   if (cudaMemsetAsync(grad_h_in, 0, (size_t)B * h * w * C * sizeof(float), s) != cudaSuccess) {
     set_error("hidden_warp_backward: memset failed");
