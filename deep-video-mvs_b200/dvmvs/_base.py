@@ -102,14 +102,14 @@ def graphed_call(owner_key, fn, args, kwargs, keep=None):
         with torch.cuda.device(dev), torch.no_grad():
             e.static_in = [torch.empty_strided(tuple(t.shape), tuple(t.stride()), dtype=t.dtype, device=t.device) for t in tensors]
             side.wait_stream(cur)
-            with torch.cuda.stream(side):
+            with torch.cuda.stream(side), ops.stand_in_for(cur):
                 torch._foreach_copy_(e.static_in, tensors)
                 a, k = _unflatten(spec, iter(e.static_in))
                 for _ in range(2):                       # warm-up: allocations, weight packing, function attributes, scratch buffers
                     fn(*a, **k)
             side.synchronize()
             g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, stream=side):
+            with torch.cuda.graph(g, stream=side), ops.stand_in_for(cur):
                 a, k = _unflatten(spec, iter(e.static_in))
                 out = fn(*a, **k)
             outs = []

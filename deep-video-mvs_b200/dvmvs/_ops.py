@@ -57,13 +57,33 @@ def on_tensor_device(fn):
 
 _WORKSPACE = {}
 WORKSPACE_BYTES = 32 << 20
+_STAND_IN = __import__("threading").local()
+
+
+class stand_in_for:
+    """Context manager: work enqueued inside runs on a stream that stands in for `stream` -- the side stream of a Fork, the
+    capture stream of an auto-graph -- and gets a split-K workspace of its own.  torch hands out its pooled streams
+    round-robin, so a stand-in can be the very CUDA stream an engine stage runs on; keyed by the stream alone, the stage's
+    graph and the stand-in's graph (replayed on another stream) would share partial sums while running concurrently."""
+
+    def __init__(self, stream):
+        self.tag = stream.cuda_stream
+
+    def __enter__(self):
+        self.prev = getattr(_STAND_IN, "tags", ())
+        _STAND_IN.tags = self.prev + (self.tag,)
+
+    def __exit__(self, *exc):
+        _STAND_IN.tags = self.prev
+        return False
 
 
 def workspace(device):
     """Scratch for the deterministic split-K reductions of small-map convolutions: one buffer per (device, stream) --
     kernels on different streams (the two stages of PipelinedFusionnet, or a user's own streams) may run concurrently
-    and must not share partial-sum storage.  Allocated once per stream."""
-    key = (device.type, device.index, 0 if N.DRYRUN else torch.cuda.current_stream(device).cuda_stream)
+    and must not share partial-sum storage.  Allocated once per stream (and per stand_in_for chain on it)."""
+    key = (device.type, device.index, 0 if N.DRYRUN else torch.cuda.current_stream(device).cuda_stream,
+           getattr(_STAND_IN, "tags", ()))
     ws = _WORKSPACE.get(key)
     if ws is None:
         # zero-initialised: its first 16 KiB hold the split-K arrival counters of conv_tc_kernel (self-cleaning)
@@ -835,12 +855,15 @@ class Fork:
             self.side.wait_event(ev)
             self._ctx = torch.cuda.stream(self.side)
             self._ctx.__enter__()
+            self._tag = stand_in_for(self.main)
+            self._tag.__enter__()
         return self
 
     def __exit__(self, *exc):
         if self.active:
             self._done = torch.cuda.Event()
             self._done.record(self.side)
+            self._tag.__exit__(*exc)
             self._ctx.__exit__(*exc)
         return False
 

@@ -280,14 +280,17 @@ def _capture_graph(fn, stream, pdl=None, state=None, depth=None):
     return g, res, n
 
 
-def _after_caller(first, last, device, frame, out):
-    """The inputs were produced on the caller's stream: orders the engine's first stream after it and keeps CUDA inputs
-    (and a CUDA `out`, written on the last stream) alive, caching-allocator wise, until the engine's work on them has run."""
-    reference_image, reference_pose, measurement_images, measurement_poses, full_K = frame
-    first.wait_stream(torch.cuda.current_stream(device))
-    for t_in in [reference_image, reference_pose, full_K] + list(measurement_images) + list(measurement_poses):
-        if t_in is not None and t_in.is_cuda:
-            t_in.record_stream(first)
+def _take_inputs(slot, frame, reuse, first, last, device, out, hits=None):
+    """Consumes one keyframe's inputs on the caller's current stream, where they were produced: that stream waits for
+    `reuse` (the event after which the static buffers of `slot` may be rewritten; None: no wait), copies the inputs into
+    them and the engine's first stream is ordered after it.  So work the caller enqueues later on its stream runs after
+    the copies: it may overwrite or free CUDA inputs, and pinned host inputs may be rewritten once that stream has passed
+    this point.  A CUDA `out`, written on the last stream, is kept alive (caching-allocator wise) until that write has run."""
+    caller = torch.cuda.current_stream(device)
+    if reuse is not None:
+        caller.wait_event(reuse)
+    _upload(slot, frame, hits)
+    first.wait_stream(caller)
     if out is not None and out.is_cuda:
         out.record_stream(last)
 
@@ -561,6 +564,11 @@ class PipelinedFusionnet:
         """Enqueue keyframe t (inputs CPU-pinned or CUDA).  If `out` (pinned host or CUDA tensor (B,H,W)) is given the
         depth is copied into it on the last stage's stream; otherwise read eng.depth_of(t) after synchronisation.
 
+        The engine behaves as if it had consumed its inputs on the caller's current stream at the time of submit(): work
+        the caller enqueues later on that stream may overwrite or free the CUDA inputs, and pinned host inputs may be
+        rewritten once that stream has passed the submit() (e.g. after torch.cuda.current_stream().synchronize()).  That
+        stream also waits, at submit(), until the slot keyframe t - n_stages used has left the pipeline.
+
         Engines built with feature_cache=N take frame ids: `measurement_ids[m]` names measurement frame m, `reference_id`
         the reference frame.  A measurement frame whose id is in the cache needs no image (pass None): its features are
         copied from the ring; on a miss the features are computed from the image (eagerly, on the sweep stage's stream)
@@ -580,15 +588,14 @@ class PipelinedFusionnet:
         elif reference_id is not None or measurement_ids is not None:
             raise ValueError("frame ids given but the engine was built without feature_cache")
         frame = (reference_image, reference_pose, measurement_images, measurement_poses, full_K)
-        _after_caller(self.streams[0], self.streams[last], self.device, frame, out)
+        # slot reuse: keyframe t-n has left the pipeline
+        _take_inputs(slot, frame, slot["done"][last], self.streams[0], self.streams[last], self.device, out, hits)
+        slot["t"] = self.t
         for i in range(n):
             stream = self.streams[i]
             key = with_state if i == last else False
             with torch.cuda.stream(stream):
-                if i == 0:
-                    stream.wait_event(slot["done"][last])         # slot reuse: keyframe t-n has left the pipeline
-                    _upload(slot, frame, hits)
-                else:
+                if i > 0:
                     stream.wait_event(slot["done"][i - 1])
                 if hits is not None and i == self._sweep_stage:
                     self._fill_measurement_features(slot, measurement_ids, hits)
@@ -636,7 +643,12 @@ class PipelinedFusionnet:
             self.cache.hits = self.cache.misses = 0
 
     def depth_of(self, t):
-        return self.slots[t % self.n_stages]["depth"]
+        """The (B,H,W) depth buffer of keyframe t, valid after synchronisation until keyframe t + n_stages is submitted.
+        Raises KeyError for a t its slot no longer (or not yet) holds."""
+        slot = self.slots[t % self.n_stages]
+        if slot.get("t") != t:
+            raise KeyError("keyframe %r: its slot holds keyframe %r" % (t, slot.get("t")))
+        return slot["depth"]
 
     def flush(self):
         """Nothing is ever held back by this engine (LookaheadFusionnet buffers keyframes; same call there launches them)."""
@@ -710,8 +722,7 @@ class LookaheadFusionnet:
         self._static_state = _StaticState()
         self._has_state = False
         self._gi, self._fill = 0, 0          # group counter, keyframes buffered in the open group
-        self._pending = []                   # (kslot index, with_state, out) of the open group
-        self._kslot_of = {}
+        self._pending = []                   # (kslot index, with_state, out, t) of the open group
         self.t = 0
         self._kernels = [0] * 5
         self.kernels_per_keyframe = 0
@@ -744,21 +755,21 @@ class LookaheadFusionnet:
     # -- steady state ---------------------------------------------------------------------------------------------------
     def submit(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K, out=None):
         """Buffer keyframe t (inputs CPU-pinned or CUDA): its inputs are copied now, its stages are launched when its group of
-        `lookahead` keyframes is complete (or at flush() / synchronize()).  `out` as in PipelinedFusionnet.submit."""
+        `lookahead` keyframes is complete (or at flush() / synchronize()).  `out` as in PipelinedFusionnet.submit.
+
+        The engine behaves as if it had consumed its inputs on the caller's current stream at the time of submit(): work
+        the caller enqueues later on that stream may overwrite or free the CUDA inputs, and pinned host inputs may be
+        rewritten once that stream has passed the submit() (e.g. after torch.cuda.current_stream().synchronize()).  At the
+        first submit() of a group that stream also waits until the group's previous use has finished."""
         g = self._gi % self.G
         grp = self.groups[g]
         ki = g * self.T + self._fill
-        s0 = self.streams[0]
         frame = (reference_image, reference_pose, measurement_images, measurement_poses, full_K)
-        _after_caller(s0, self.streams[4], self.device, frame, out)
-        with torch.cuda.stream(s0):
-            if self._fill == 0:
-                s0.wait_event(grp["rec_done"])           # every stage of this group's previous use has finished reading its buffers
-            _upload(self.kslots[ki], frame)
-        self._pending.append((ki, self._has_state, out))
+        # group reuse: every stage of this group's previous use has finished reading its buffers
+        _take_inputs(self.kslots[ki], frame, grp["rec_done"] if self._fill == 0 else None, self.streams[0], self.streams[4],
+                     self.device, out)
+        self._pending.append((ki, self._has_state, out, self.t))
         self._has_state = True
-        self._kslot_of[self.t] = ki
-        self._kslot_of.pop(self.t - 4 * self.T * self.G, None)
         self._fill += 1
         self.t += 1
         if self._fill == self.T:
@@ -790,8 +801,9 @@ class LookaheadFusionnet:
         run(1, s1, lambda: self.mods["fpn"](*self.mods["fe"].forward_tail(grp["head"])), "pyramid", grp["done"][0])
         run(2, s2, lambda: _sweep_from_pyramid(grp, grp["pyramid"], 0, *self.depth_args), "swept", grp["done"][1])
         run(3, s3, lambda: _stage_enc(self.mods, grp, grp["swept"]), "enc", grp["done"][2])
-        for ki, with_state, out in self._pending:
+        for ki, with_state, out, t in self._pending:
             ks = self.kslots[ki]
+            ks["t"] = t
             with torch.cuda.stream(s4):
                 s4.wait_event(grp["done"][3])
                 if with_state not in ks["graph"]:
@@ -815,7 +827,13 @@ class LookaheadFusionnet:
         self.reset()
 
     def depth_of(self, t):
-        return self.kslots[self._kslot_of[t]]["depth"]
+        """The (B,H,W) depth buffer of keyframe t, valid after synchronisation from the launch of its group (flush()) until
+        the launch of the next keyframe in its slot.  Raises KeyError for a t no slot holds: stale, not yet submitted, or
+        buffered in a group not launched yet."""
+        for ks in self.kslots:
+            if ks.get("t") == t:
+                return ks["depth"]
+        raise KeyError("keyframe %r: no keyframe slot holds its depth" % (t,))
 
     def synchronize(self):
         self.flush()

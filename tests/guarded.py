@@ -512,9 +512,9 @@ def guard_allocations(modules=None, device_type="cuda", guard_arguments=True):
                     setattr(L, sym, _record_native(sym, getattr(L, sym)))
         if device_type == "cuda":
             dev = torch.device("cuda", torch.cuda.current_device())
-            key = (dev.type, dev.index, 0 if N.DRYRUN else torch.cuda.current_stream(dev).cuda_stream)
+            key = (dev.type, dev.index, 0 if N.DRYRUN else torch.cuda.current_stream(dev).cuda_stream, ())
         else:
-            dev, key = torch.device(device_type), (device_type, None, 0)
+            dev, key = torch.device(device_type), (device_type, None, 0, ())
         ws = _alloc((_ops.WORKSPACE_BYTES // 4,), torch.float32, dev, WORKSPACE, "split-K workspace")
         _ops._WORKSPACE = {key: ws.view}      # workspaces of other streams are created on demand through the proxy
         REGISTRY.workspaces = _ops._WORKSPACE
