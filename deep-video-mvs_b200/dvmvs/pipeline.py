@@ -658,6 +658,53 @@ class PipelinedFusionnet:
             s.synchronize()
 
 
+def _group_buffers(T, B, H, W, M, device):
+    """Input buffers of one group of T keyframes x B clips (TB = T * B rows) of a lookahead engine: the images stacked
+    [reference block | measurement 1 block | ...], TB rows each, and the poses and intrinsics per row, sane until a keyframe
+    overwrites them (identity poses, a valid K), so that the rows of an incomplete group always hold finite inputs."""
+    TB = T * B
+    images = torch.zeros(((M + 1) * TB, 3, H, W), dtype=torch.float32, device=device)
+    K0 = torch.tensor([[float(W), 0.0, W / 2.0], [0.0, float(W), H / 2.0], [0.0, 0.0, 1.0]], device=device).repeat(TB, 1, 1)
+    eye = lambda: torch.eye(4, dtype=torch.float32, device=device).repeat(TB, 1, 1)
+    return {"images": images, "ref_image": images[:TB], "meas_images": [images[(m + 1) * TB:(m + 2) * TB] for m in range(M)],
+            "ref_pose": eye(), "full_K": K0, "meas_poses": [eye() for _ in range(M)]}
+
+
+def _keyframe_rows(grp, j, B):
+    """Keyframe j's rows lo:hi of every input block of a group: the views _upload writes its inputs into."""
+    lo, hi = j * B, (j + 1) * B
+    return {"lo": lo, "hi": hi, "ref_image": grp["ref_image"][lo:hi], "meas_images": [mi[lo:hi] for mi in grp["meas_images"]],
+            "ref_pose": grp["ref_pose"][lo:hi], "full_K": grp["full_K"][lo:hi], "meas_poses": [mp[lo:hi] for mp in grp["meas_poses"]]}
+
+
+def _group_head(mods, grp):
+    """MnasNet trunk up to layer3 over all (M + 1) x TB images of a group, after the side inputs of the later stages (channel-last
+    reference images, 1/32 intrinsics)."""
+    _stage_side_inputs(grp)
+    return mods["fe"].forward_head(grp["images"])
+
+
+def _group_stages(mods, depth_args):
+    """(key, body) of the stages both lookahead engines run over a whole group, in stream order: trunk head | trunk tail +
+    feature pyramid | plane sweep (each row with its own poses) | cost-volume encoder.  body(grp) reads the outputs earlier
+    stages left in grp under their keys; its result is stored under `key`."""
+    return [("head", lambda grp: _group_head(mods, grp)),
+            ("pyramid", lambda grp: mods["fpn"](*mods["fe"].forward_tail(grp["head"]))),
+            ("swept", lambda grp: _sweep_from_pyramid(grp, grp["pyramid"], 0, *depth_args)),
+            ("enc", lambda grp: _stage_enc(mods, grp, grp["swept"]))]
+
+
+def _group_decode(mods, grp):
+    """Pairnet's decoder over a whole group: the (TB, H, W) depth, keyframe j's in rows j*B:(j+1)*B."""
+    enc, _ = grp["enc"]
+    return mods["cvd"](grp["ref_cl"], *enc)[0]
+
+
+def _pairnet_group_stages(mods, depth_args):
+    """LookaheadPairnet's five stages: _group_stages, then the decoder over the group (no recurrent state to serialise on)."""
+    return _group_stages(mods, depth_args) + [("depth", lambda grp: _group_decode(mods, grp))]
+
+
 class LookaheadFusionnet:
     """Throughput engine with everything that does NOT depend on the recurrent state batched over TIME: FeatureExtractor,
     FeatureShrinker, the plane sweep and the cost-volume encoder run once per group of `lookahead` consecutive keyframes
@@ -692,25 +739,16 @@ class LookaheadFusionnet:
         dev = device or next(mods["fe"].parameters()).device
         self.device = dev
         self.T, self.G = int(lookahead), int(n_groups)
-        TB = self.T * batch
         z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
-        eye = lambda: torch.eye(4, dtype=torch.float32, device=dev).repeat(TB, 1, 1)
         self.groups, self.kslots = [], []
         for g in range(self.G):
-            images = z((n_measurement_frames + 1) * TB, 3, height, width)      # [reference block | measurement 1 block | ...], TB rows each
-            K0 = torch.tensor([[float(width), 0.0, width / 2.0], [0.0, float(width), height / 2.0], [0.0, 0.0, 1.0]], device=dev).repeat(TB, 1, 1)
-            grp = {"images": images, "ref_image": images[:TB],
-                   "meas_images": [images[(m + 1) * TB:(m + 2) * TB] for m in range(n_measurement_frames)],
-                   "ref_pose": eye(), "full_K": K0, "meas_poses": [eye() for _ in range(n_measurement_frames)],   # sane until overwritten
-                   "head": None, "pyramid": None, "swept": None, "enc": None, "graph": [None] * 4,
-                   "done": [torch.cuda.Event() for _ in range(4)], "rec_done": torch.cuda.Event()}
+            grp = _group_buffers(self.T, batch, height, width, n_measurement_frames, dev)
+            grp.update({"head": None, "pyramid": None, "swept": None, "enc": None, "graph": [None] * 4,
+                        "done": [torch.cuda.Event() for _ in range(4)], "rec_done": torch.cuda.Event()})
             self.groups.append(grp)
             for j in range(self.T):
-                lo, hi = j * batch, (j + 1) * batch
-                self.kslots.append({"group": g, "lo": lo, "hi": hi, "ref_image": grp["ref_image"][lo:hi],
-                                    "meas_images": [mi[lo:hi] for mi in grp["meas_images"]], "ref_pose": grp["ref_pose"][lo:hi],
-                                    "full_K": grp["full_K"][lo:hi], "meas_poses": [mp[lo:hi] for mp in grp["meas_poses"]],
-                                    "depth": z(batch, height, width), "graph": dict(), "done": torch.cuda.Event()})
+                self.kslots.append(dict(_keyframe_rows(grp, j, batch), group=g, depth=z(batch, height, width), graph=dict(),
+                                        done=torch.cuda.Event()))
         # the recurrent stage's small kernels carry the loop dependence; on a high-priority stream their CTAs are dispatched
         # ahead of the queued CTAs of the batched stages' big grids (DVMVS_LA_PRIO=0: all streams equal)
         prio = os.environ.get("DVMVS_LA_PRIO", "1") == "1"
@@ -782,25 +820,16 @@ class LookaheadFusionnet:
         if not self._pending:
             return
         grp = self.groups[self._gi % self.G]
-        s0, s1, s2, s3, s4 = self.streams
-
-        def run(i, stream, fn, key, after):
+        s4 = self.streams[4]
+        for i, (key, body) in enumerate(_group_stages(self.mods, self.depth_args)):
+            stream = self.streams[i]
             with torch.cuda.stream(stream):
-                if after is not None:
-                    stream.wait_event(after)
+                if i > 0:
+                    stream.wait_event(grp["done"][i - 1])
                 if grp["graph"][i] is None:
-                    grp["graph"][i], grp[key], self._kernels[i] = self._capture(fn, stream)
+                    grp["graph"][i], grp[key], self._kernels[i] = self._capture(lambda: body(grp), stream)
                 grp["graph"][i].replay()
                 grp["done"][i].record(stream)
-
-        def head_fn():
-            _stage_side_inputs(grp)                  # channel-last reference images + 1/32 intrinsics for the recurrent stage
-            return self.mods["fe"].forward_head(grp["images"])
-
-        run(0, s0, head_fn, "head", None)
-        run(1, s1, lambda: self.mods["fpn"](*self.mods["fe"].forward_tail(grp["head"])), "pyramid", grp["done"][0])
-        run(2, s2, lambda: _sweep_from_pyramid(grp, grp["pyramid"], 0, *self.depth_args), "swept", grp["done"][1])
-        run(3, s3, lambda: _stage_enc(self.mods, grp, grp["swept"]), "enc", grp["done"][2])
         for ki, with_state, out, t in self._pending:
             ks = self.kslots[ki]
             ks["t"] = t
@@ -825,6 +854,130 @@ class LookaheadFusionnet:
             self.submit(reference_image, reference_pose, measurement_images, measurement_poses, full_K)
         self.synchronize()
         self.reset()
+
+    def depth_of(self, t):
+        """The (B,H,W) depth buffer of keyframe t, valid after synchronisation from the launch of its group (flush()) until
+        the launch of the next keyframe in its slot.  Raises KeyError for a t no slot holds: stale, not yet submitted, or
+        buffered in a group not launched yet."""
+        for ks in self.kslots:
+            if ks.get("t") == t:
+                return ks["depth"]
+        raise KeyError("keyframe %r: no keyframe slot holds its depth" % (t,))
+
+    def synchronize(self):
+        self.flush()
+        for s in self.streams:
+            s.synchronize()
+
+
+class LookaheadPairnet:
+    """LookaheadFusionnet's throughput engine for pairnet modules (build_modules(..., pairnet=True)).  Pairnet carries no state
+    from one keyframe to the next, so the decoder runs batched over time too: every stage -- trunk head | trunk tail + feature
+    pyramid | plane sweep | cost-volume encoder | decoder -- is one CUDA graph per group of `lookahead` x B keyframes, on its
+    own stream, chained by per-group events.  Every keyframe still gets all of its M + 1 feature passes (no feature cache).
+    Same API as LookaheadFusionnet minus load_state, so a caller can swap one for the other:
+
+        eng = LookaheadPairnet(mods, batch=B, height=H, width=W, n_measurement_frames=M, lookahead=4)
+        for frame in stream:  eng.submit(*frame, out=pinned_host_tensor_or_None)
+        eng.synchronize()
+
+    Each batch row is computed on its own, so a keyframe's depth does not depend on its neighbours in the group; against
+    keyframe() the results differ only by the split-K choice of a few convolutions, which depends on the batch."""
+
+    n_stages = 5
+
+    def __init__(self, mods, batch, height, width, n_measurement_frames, min_depth=0.25, max_depth=20.0, n_depth_levels=64,
+                 device=None, lookahead=4, n_groups=3):
+        if "lstm" in mods:
+            raise ValueError("LookaheadPairnet runs pairnet modules; fusionnet modules (with 'lstm') go to LookaheadFusionnet")
+        if lookahead < 1 or n_groups < 2:
+            raise ValueError("lookahead >= 1 and n_groups >= 2 required")
+        self.mods, self.B, self.H, self.W, self.M = mods, batch, height, width, n_measurement_frames
+        self.depth_args = (min_depth, max_depth, n_depth_levels)
+        dev = device or next(mods["fe"].parameters()).device
+        self.device = dev
+        self.T, self.G = int(lookahead), int(n_groups)
+        z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
+        self.groups, self.kslots = [], []
+        for g in range(self.G):
+            grp = _group_buffers(self.T, batch, height, width, n_measurement_frames, dev)
+            grp.update({"graph": [None] * 5, "done": [torch.cuda.Event() for _ in range(5)]})
+            self.groups.append(grp)
+            for j in range(self.T):
+                self.kslots.append(dict(_keyframe_rows(grp, j, batch), group=g, depth=z(batch, height, width)))
+        self.stages = _pairnet_group_stages(mods, self.depth_args)
+        # no loop-carried stage to favour: all streams at the same priority
+        self.streams = [torch.cuda.Stream(device=dev) for _ in range(5)]
+        self.stream_a, self.stream_b = self.streams[0], self.streams[-1]
+        self._gi, self._fill = 0, 0          # group counter, keyframes buffered in the open group
+        self._pending = []                   # (kslot index, out, t) of the open group
+        self.t = 0
+        self._kernels = [0] * 5
+        self.kernels_per_keyframe = 0
+
+    def reset(self):
+        """Does nothing: pairnet keyframes carry no state from one to the next, so there is no clip state to drop.  Kept so
+        that code written for LookaheadFusionnet (reset() at a new clip or on tracking loss) runs unchanged."""
+
+    def submit(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K, out=None):
+        """Buffer keyframe t (inputs CPU-pinned or CUDA): its inputs are copied now, its group's stages are launched when the
+        group of `lookahead` keyframes is complete (or at flush() / synchronize()).  If `out` (pinned host or CUDA tensor
+        (B,H,W)) is given, the depth is copied into it on the decoder's stream; otherwise read eng.depth_of(t).
+
+        The engine behaves as if it had consumed its inputs on the caller's current stream at the time of submit(): work
+        the caller enqueues later on that stream may overwrite or free the CUDA inputs, and pinned host inputs may be
+        rewritten once that stream has passed the submit() (e.g. after torch.cuda.current_stream().synchronize()).  At the
+        first submit() of a group that stream also waits until the decoder stage of the group's previous use has finished."""
+        g = self._gi % self.G
+        grp = self.groups[g]
+        ki = g * self.T + self._fill
+        frame = (reference_image, reference_pose, measurement_images, measurement_poses, full_K)
+        # group reuse: the decoder stage of this group's previous use ran after every other stage of that use
+        _take_inputs(self.kslots[ki], frame, grp["done"][4] if self._fill == 0 else None, self.streams[0], self.streams[4],
+                     self.device, out)
+        self._pending.append((ki, out, self.t))
+        self._fill += 1
+        self.t += 1
+        if self._fill == self.T:
+            self.flush()
+        return self.t - 1
+
+    def flush(self):
+        """Launch the open group (complete or not): the five stages over the group's buffers, then each buffered keyframe's
+        rows of the group's depth copied into its own depth buffer (and `out`).  Rows no keyframe filled keep the finite
+        inputs they held before; their results are not read."""
+        if not self._pending:
+            return
+        grp = self.groups[self._gi % self.G]
+        for i, (key, body) in enumerate(self.stages):
+            stream = self.streams[i]
+            with torch.cuda.stream(stream):
+                if i > 0:
+                    stream.wait_event(grp["done"][i - 1])
+                if grp["graph"][i] is None:
+                    torch.cuda.synchronize(self.device)
+                    grp["graph"][i], grp[key], self._kernels[i] = _capture_graph(lambda: body(grp), stream, False)
+                    torch.cuda.synchronize(self.device)
+                grp["graph"][i].replay()
+                if i == 4:
+                    for ki, out, t in self._pending:
+                        ks = self.kslots[ki]
+                        ks["t"] = t
+                        ks["depth"].copy_(grp["depth"][ks["lo"]:ks["hi"]], non_blocking=True)
+                        if out is not None:
+                            out.copy_(ks["depth"], non_blocking=True)
+                grp["done"][i].record(stream)
+        self.kernels_per_keyframe = sum(self._kernels) / float(self.T)      # a full group's launches per keyframe
+        self._pending = []
+        self._fill = 0
+        self._gi += 1
+
+    def prime(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K):
+        """Captures every group's graphs with n_groups x lookahead throw-away keyframes, so that the one-off captures stay out
+        of a timed or latency-sensitive region."""
+        for _ in range(self.G * self.T):
+            self.submit(reference_image, reference_pose, measurement_images, measurement_poses, full_K)
+        self.synchronize()
 
     def depth_of(self, t):
         """The (B,H,W) depth buffer of keyframe t, valid after synchronisation from the launch of its group (flush()) until
