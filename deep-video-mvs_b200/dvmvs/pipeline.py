@@ -55,50 +55,84 @@ class FeatureCache:
     features are the same numbers; this cache keeps them in a fixed ring of device buffers (FIFO eviction, capacity =
     the keyframe buffer size, Config.test_keyframe_buffer_size) and hands them back.  Ids are explicit because the scripts
     re-upload the images as fresh tensors each keyframe: nothing on the device identifies a frame without a host sync.
-    A miss is not an error -- the caller computes the features from the image and stores them."""
+    A miss is not an error -- the caller computes the features from the image and stores them.
+
+    The ring is one device tensor `ring` of capacity + 1 entries (B, h, w, 32), so that a device index tensor can address
+    it inside a CUDA graph (the lookahead engines store and gather whole groups with one indexed copy each).  Entry
+    `capacity` is a sink no frame id owns: rows of an incomplete group that no keyframe filled store to it and gather from
+    it.  Those engines reserve() entries at submit(); a reserved entry is pinned until unpin(), and FIFO eviction skips
+    pinned entries."""
 
     def __init__(self, capacity=30):
         if capacity < 1:
             raise ValueError("FeatureCache capacity must be >= 1")
         self.capacity = int(capacity)
-        self._ring = [None] * self.capacity      # (B, h, w, 32) channel-last buffers, allocated on first use
+        self.sink = self.capacity
+        self.ring = None                          # (capacity + 1, B, h, w, 32), allocated by allocate() or the first store
         self._index = {}                          # frame id -> ring index
         self._owner = [None] * self.capacity
-        self._next = 0
+        self._pinned = set()
         self.hits = 0
         self.misses = 0
+
+    def allocate(self, entry_shape, device):
+        """Allocates the ring for entries of shape (B, h, w, 32) on `device` (zeros: the sink gathers finite values)."""
+        self.ring = torch.zeros((self.capacity + 1,) + tuple(entry_shape), dtype=torch.float32, device=device)
 
     def clear(self):
         self._index.clear()
         self._owner = [None] * self.capacity
+        self._pinned.clear()
 
     def __contains__(self, frame_id):
         return frame_id in self._index
 
+    def _entry(self, frame_id):
+        """Ring index of `frame_id`; a new id takes a free entry or, with the ring full, evicts the oldest id (FIFO, in the
+        order ids entered; a re-stored id keeps its age) whose entry no reservation pins."""
+        idx = self._index.get(frame_id)
+        if idx is None:
+            if len(self._index) < self.capacity:
+                idx = self._owner.index(None)
+            else:
+                victim = next((fid for fid, i in self._index.items() if i not in self._pinned), None)
+                if victim is None:
+                    raise RuntimeError("feature cache: every entry is pinned")
+                idx = self._index.pop(victim)
+            self._owner[idx] = frame_id
+            self._index[frame_id] = idx
+        return idx
+
     def lookup(self, frame_id):
-        """Cached (B,32,h,w) API tensor (channels_last view of the ring buffer) or None."""
+        """Cached (B,32,h,w) API tensor (channels_last view of the ring entry) or None."""
         idx = self._index.get(frame_id)
         if idx is None:
             self.misses += 1
             return None
         self.hits += 1
-        return self._ring[idx].permute(0, 3, 1, 2)
+        return self.ring[idx].permute(0, 3, 1, 2)
 
     def store(self, frame_id, half_features):
         """Copies (B,32,h,w) features into the ring on the current stream (a D2D copy; the ring outlives the caller's tensor)."""
-        idx = self._index.get(frame_id)
-        if idx is None:
-            idx = self._next
-            self._next = (self._next + 1) % self.capacity
-            if self._owner[idx] is not None:
-                del self._index[self._owner[idx]]
-            self._owner[idx] = frame_id
-            self._index[frame_id] = idx
         src = half_features.permute(0, 2, 3, 1)
-        if self._ring[idx] is None or self._ring[idx].shape != src.shape or self._ring[idx].device != src.device:
-            self._ring[idx] = torch.empty(tuple(src.shape), dtype=torch.float32, device=src.device)
-        self._ring[idx].copy_(src)
+        if self.ring is None:
+            self.allocate(src.shape, src.device)
+        elif self.ring.shape[1:] != src.shape or self.ring.device != src.device:
+            raise ValueError("feature cache holds entries of shape %s on %s, got %s on %s"
+                             % (tuple(self.ring.shape[1:]), self.ring.device, tuple(src.shape), src.device))
+        idx = self._entry(frame_id)
+        self.ring[idx].copy_(src)
         return idx
+
+    def reserve(self, frame_id):
+        """The ring entry `frame_id` is (or, if absent, will be) stored in, pinned until unpin(): no reservation or store
+        evicts it before then.  Nothing is copied; the caller fills a new entry."""
+        idx = self._entry(frame_id)
+        self._pinned.add(idx)
+        return idx
+
+    def unpin(self):
+        self._pinned.clear()
 
 
 def _plane_sweep(f2, meas_half, ref_pose, meas_poses, full_K, min_depth, max_depth, n_depth_levels):
@@ -280,16 +314,19 @@ def _capture_graph(fn, stream, pdl=None, state=None, depth=None):
     return g, res, n
 
 
-def _take_inputs(slot, frame, reuse, first, last, device, out, hits=None):
+def _take_inputs(slot, frame, reuse, first, last, device, out, hits=None, ring_index=None):
     """Consumes one keyframe's inputs on the caller's current stream, where they were produced: that stream waits for
     `reuse` (the event after which the static buffers of `slot` may be rewritten; None: no wait), copies the inputs into
     them and the engine's first stream is ordered after it.  So work the caller enqueues later on its stream runs after
     the copies: it may overwrite or free CUDA inputs, and pinned host inputs may be rewritten once that stream has passed
-    this point.  A CUDA `out`, written on the last stream, is kept alive (caching-allocator wise) until that write has run."""
+    this point.  A CUDA `out`, written on the last stream, is kept alive (caching-allocator wise) until that write has run.
+    ring_index: (device buffer, host tensor) of a lookahead engine's feature-cache ring indices, copied with the inputs."""
     caller = torch.cuda.current_stream(device)
     if reuse is not None:
         caller.wait_event(reuse)
     _upload(slot, frame, hits)
+    if ring_index is not None:
+        ring_index[0].copy_(ring_index[1], non_blocking=True)
     first.wait_stream(caller)
     if out is not None and out.is_cuda:
         out.record_stream(last)
@@ -307,6 +344,23 @@ def _upload(slot, frame, hits=None):
             dst.copy_(src, non_blocking=True)
     for dst, src in zip(slot["meas_poses"], measurement_poses):
         dst.copy_(src, non_blocking=True)
+
+
+def _cache_hits(cache, M, measurement_images, reference_id, measurement_ids):
+    """The frame-id rules of submit() for the engines with a feature cache, checked before anything is copied or launched:
+    ids only with a cache, one id per measurement frame, and an image for every measurement frame the cache does not hold.
+    Returns hits[m] (measurement frame m is cached), or None for an engine without a cache."""
+    if cache is None:
+        if reference_id is not None or measurement_ids is not None:
+            raise ValueError("frame ids given but the engine was built without feature_cache")
+        return None
+    if measurement_ids is None or len(measurement_ids) != M:
+        raise ValueError("feature cache: need %d measurement frame ids" % M)
+    hits = [i in cache for i in measurement_ids]
+    for m, hit in enumerate(hits):
+        if not hit and measurement_images[m] is None:
+            raise ValueError("feature cache miss for frame id %r and no image given" % (measurement_ids[m],))
+    return hits
 
 
 def _load_state(self, lstm_state, previous_depth, previous_pose):
@@ -576,17 +630,7 @@ class PipelinedFusionnet:
         n, last = self.n_stages, self.n_stages - 1
         slot = self.slots[self.t % n]
         with_state = self._has_state
-        hits = None
-        if self.cache is not None:
-            if measurement_ids is None or len(measurement_ids) != self.M:
-                raise ValueError("feature cache: need %d measurement frame ids" % self.M)
-            hits = [i in self.cache for i in measurement_ids]
-            measurement_images = list(measurement_images)
-            for m, hit in enumerate(hits):
-                if not hit and measurement_images[m] is None:
-                    raise ValueError("feature cache miss for frame id %r and no image given" % (measurement_ids[m],))
-        elif reference_id is not None or measurement_ids is not None:
-            raise ValueError("frame ids given but the engine was built without feature_cache")
+        hits = _cache_hits(self.cache, self.M, measurement_images, reference_id, measurement_ids)
         frame = (reference_image, reference_pose, measurement_images, measurement_poses, full_K)
         # slot reuse: keyframe t-n has left the pipeline
         _take_inputs(slot, frame, slot["done"][last], self.streams[0], self.streams[last], self.device, out, hits)
@@ -677,20 +721,94 @@ def _keyframe_rows(grp, j, B):
             "ref_pose": grp["ref_pose"][lo:hi], "full_K": grp["full_K"][lo:hi], "meas_poses": [mp[lo:hi] for mp in grp["meas_poses"]]}
 
 
+def _ring_buffers(grp, cache, T, B, H, W, M):
+    """The feature-cache buffers of one group of a lookahead engine: `meas_half`, every keyframe's gathered measurement
+    features in the [M][T][B] row order of the measurement image blocks (M views of TB channel-last rows), and `ring_index`,
+    the ring entries the group's sweep stage addresses: row 0 the entry each keyframe's reference features are stored in,
+    row 1 + m the entry measurement frame m is gathered from.  `ring_table` is its host copy, rewritten at each submit();
+    columns no keyframe filled name the sink."""
+    device = cache.ring.device
+    grp["meas_half_rows"] = torch.zeros((M * T, B, H // 2, W // 2, 32), dtype=torch.float32, device=device)
+    grp["meas_half"] = [grp["meas_half_rows"][m * T:(m + 1) * T].view(T * B, H // 2, W // 2, 32) for m in range(M)]
+    grp["ring_index"] = torch.full((M + 1, T), cache.sink, dtype=torch.int64, device=device)
+    grp["ring_table"] = torch.full((M + 1, T), cache.sink, dtype=torch.int64)
+    grp["misses"] = []                    # (keyframe j, measurement m, ring entry) to compute at flush()
+
+
+def _reserve_keyframe(cache, grp, j, reference_id, measurement_ids, hits):
+    """Reserves (and pins) the ring entries keyframe j of the open group reads and stores, writes them into column j of the
+    group's host index table, and counts the hits and misses.  Hits are pinned first, so that the entries taken for
+    the misses and the reference frame cannot evict them.
+
+    Why evicting here is safe: every ring write and every ring read runs on the sweep stage's stream, in group order --
+    the miss stores flush() computes just before the sweep stage's graph, then that graph's store of the reference
+    features and its gather of the measurement features.  An entry this reservation evicts can therefore still be read
+    only by groups launched earlier, whose gathers precede this group's stores on that stream, or by this group, whose
+    own entries are pinned until it is launched."""
+    if j == 0:
+        grp["ring_table"].fill_(cache.sink)
+        grp["misses"] = []
+    for want_hit in (True, False):
+        for m, hit in enumerate(hits):
+            if hit == want_hit:
+                grp["ring_table"][1 + m, j] = idx = cache.reserve(measurement_ids[m])
+                if not hit:
+                    grp["misses"].append((j, m, idx))
+    grp["ring_table"][0, j] = cache.sink if reference_id is None else cache.reserve(reference_id)
+    cache.hits += sum(hits)
+    cache.misses += len(hits) - sum(hits)
+    return grp["ring_index"], grp["ring_table"].clone()
+
+
+def _store_misses(mods, cache, grp, B):
+    """The open group's missed measurement frames: FeatureShrinker(FeatureExtractor(image)) of each, eagerly on the current
+    (the sweep stage's) stream, into its ring entry, before the sweep stage's graph gathers from the ring."""
+    for j, m, idx in grp["misses"]:
+        with torch.no_grad():
+            half, _, _, _ = mods["fpn"](*mods["fe"](grp["meas_images"][m][j * B:(j + 1) * B]))
+        cache.ring[idx].copy_(half.permute(0, 2, 3, 1))
+    grp["misses"] = []
+
+
+def _ring_store(grp, ring):
+    """Each keyframe's half-resolution reference features (its B rows of the pyramid's a2) -> its ring entry."""
+    a2 = grp["pyramid"][0]
+    T = grp["ring_index"].shape[1]
+    ring.index_copy_(0, grp["ring_index"][0], a2.permute(0, 2, 3, 1).reshape((T, -1) + tuple(ring.shape[2:])))
+
+
+def _ring_gather(grp, ring):
+    """Every keyframe's measurement features <- their ring entries, into the group's `meas_half` rows."""
+    torch.index_select(ring, 0, grp["ring_index"][1:].reshape(-1), out=grp["meas_half_rows"])
+
+
+def _ring_sweep(grp, ring, depth_args):
+    """The sweep stage of a lookahead engine with a feature cache: store, gather, then the plane sweep."""
+    _ring_store(grp, ring)
+    _ring_gather(grp, ring)
+    return _sweep_from_pyramid(grp, grp["pyramid"], 0, *depth_args)
+
+
 def _group_head(mods, grp):
-    """MnasNet trunk up to layer3 over all (M + 1) x TB images of a group, after the side inputs of the later stages (channel-last
-    reference images, 1/32 intrinsics)."""
+    """MnasNet trunk up to layer3 over all (M + 1) x TB images of a group -- the TB reference images only when the measurement
+    features come from the feature cache -- after the side inputs of the later stages (channel-last reference images, 1/32
+    intrinsics)."""
     _stage_side_inputs(grp)
-    return mods["fe"].forward_head(grp["images"])
+    return mods["fe"].forward_head(grp["ref_image"] if "meas_half" in grp else grp["images"])
 
 
-def _group_stages(mods, depth_args):
+def _group_stages(mods, depth_args, cache=None):
     """(key, body) of the stages both lookahead engines run over a whole group, in stream order: trunk head | trunk tail +
     feature pyramid | plane sweep (each row with its own poses) | cost-volume encoder.  body(grp) reads the outputs earlier
-    stages left in grp under their keys; its result is stored under `key`."""
+    stages left in grp under their keys; its result is stored under `key`.  With a feature cache the plane-sweep stage also
+    stores the reference features into the cache's ring and gathers the measurement features from it (_ring_sweep)."""
+    if cache is None:
+        sweep = lambda grp: _sweep_from_pyramid(grp, grp["pyramid"], 0, *depth_args)
+    else:
+        sweep = lambda grp: _ring_sweep(grp, cache.ring, depth_args)
     return [("head", lambda grp: _group_head(mods, grp)),
             ("pyramid", lambda grp: mods["fpn"](*mods["fe"].forward_tail(grp["head"]))),
-            ("swept", lambda grp: _sweep_from_pyramid(grp, grp["pyramid"], 0, *depth_args)),
+            ("swept", sweep),
             ("enc", lambda grp: _stage_enc(mods, grp, grp["swept"]))]
 
 
@@ -700,9 +818,27 @@ def _group_decode(mods, grp):
     return mods["cvd"](grp["ref_cl"], *enc)[0]
 
 
-def _pairnet_group_stages(mods, depth_args):
+def _pairnet_group_stages(mods, depth_args, cache=None):
     """LookaheadPairnet's five stages: _group_stages, then the decoder over the group (no recurrent state to serialise on)."""
-    return _group_stages(mods, depth_args) + [("depth", lambda grp: _group_decode(mods, grp))]
+    return _group_stages(mods, depth_args, cache) + [("depth", lambda grp: _group_decode(mods, grp))]
+
+
+def _lookahead_cache(feature_cache, T, B, H, W, M, device):
+    """The feature cache of a lookahead engine (None for feature_cache=0), its ring allocated.  One open group pins at most
+    T (M + 1) entries, so with at least that many a reservation always finds an entry to take."""
+    if not feature_cache:
+        return None
+    if feature_cache < T * (M + 1):
+        raise ValueError("feature_cache must be at least lookahead * (n_measurement_frames + 1) = %d, got %d"
+                         % (T * (M + 1), feature_cache))
+    cache = FeatureCache(feature_cache)
+    cache.allocate((B, H // 2, W // 2, 32), device)
+    return cache
+
+
+def _prime_ids(k, M):
+    """Throw-away frame ids of prime()'s k-th keyframe: all misses, so that the miss path is exercised too."""
+    return {"reference_id": ("prime", k), "measurement_ids": [("prime-m", k, m) for m in range(M)]}
 
 
 class LookaheadFusionnet:
@@ -711,7 +847,7 @@ class LookaheadFusionnet:
     (lookahead x B "clips", each with its own poses and its own M measurement frames) instead of once per keyframe; only the
     loop-carried stage (depth re-projection, ConvLSTM, decoder) runs keyframe by keyframe, on batch slices of the group's
     encoder outputs.  Every keyframe still gets all of its M + 1 feature passes, its own cost volume and its own encoder pass
-    -- nothing is cached or skipped (this is NOT the feature cache of row f1); the state-independent work is merely issued in
+    -- without feature_cache nothing is cached or skipped; the state-independent work is merely issued in
     batches the GPU runs far more efficiently than batches of one keyframe (at 8 x 8 .. 64 x 64 maps a single keyframe's
     kernels are one-tile CTAs and launch-bound).  Five streams as in PipelinedFusionnet: trunk head | trunk tail + pyramid |
     plane sweep | encoder | recurrent stage.
@@ -723,6 +859,13 @@ class LookaheadFusionnet:
     <= 1 ulp of fp32 with 3-term operands, rounding flips of the fp16 operands in 1-term mode); the parity tests hold this
     engine to the same bounds against the oracle.
 
+    feature_cache=N (row f1) keeps the half-resolution features of past reference frames in a ring of N entries (at least
+    lookahead x (M + 1)) keyed by caller-supplied frame ids, as PipelinedFusionnet(feature_cache=N) does: the trunk and the
+    feature pyramid then run over the group's reference images only, and the plane-sweep stage stores them into the ring and
+    gathers every keyframe's measurement features from it.  submit() takes reference_id / measurement_ids; a measurement
+    frame whose id the engine holds (`frame_id in eng.cache`, earlier keyframes of the open group included) needs no image
+    (pass None), a miss is computed from its image at flush().  feature_cache=0 is the engine without a cache.
+
         eng = LookaheadFusionnet(mods, batch=B, height=H, width=W, n_measurement_frames=M, lookahead=4)
         for frame in stream:  eng.submit(*frame, out=pinned_host_tensor_or_None)
         eng.synchronize()
@@ -731,7 +874,7 @@ class LookaheadFusionnet:
     n_stages = 5
 
     def __init__(self, mods, batch, height, width, n_measurement_frames, min_depth=0.25, max_depth=20.0, n_depth_levels=64,
-                 device=None, lookahead=4, n_groups=3):
+                 device=None, lookahead=4, n_groups=3, feature_cache=0):
         if lookahead < 1 or n_groups < 2:
             raise ValueError("lookahead >= 1 and n_groups >= 2 required")
         self.mods, self.B, self.H, self.W, self.M = mods, batch, height, width, n_measurement_frames
@@ -739,10 +882,13 @@ class LookaheadFusionnet:
         dev = device or next(mods["fe"].parameters()).device
         self.device = dev
         self.T, self.G = int(lookahead), int(n_groups)
+        self.cache = _lookahead_cache(feature_cache, self.T, batch, height, width, n_measurement_frames, dev)
         z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
         self.groups, self.kslots = [], []
         for g in range(self.G):
             grp = _group_buffers(self.T, batch, height, width, n_measurement_frames, dev)
+            if self.cache is not None:
+                _ring_buffers(grp, self.cache, self.T, batch, height, width, n_measurement_frames)
             grp.update({"head": None, "pyramid": None, "swept": None, "enc": None, "graph": [None] * 4,
                         "done": [torch.cuda.Event() for _ in range(4)], "rec_done": torch.cuda.Event()})
             self.groups.append(grp)
@@ -766,7 +912,8 @@ class LookaheadFusionnet:
         self.kernels_per_keyframe = 0
 
     def reset(self):
-        """New clip / tracking lost: the next submitted keyframe starts without recurrent state (buffered keyframes keep theirs)."""
+        """New clip / tracking lost: the next submitted keyframe starts without recurrent state (buffered keyframes keep theirs).
+        The feature cache is keyed by frame id and stays."""
         self._has_state = False
 
     load_state = _load_state
@@ -791,21 +938,26 @@ class LookaheadFusionnet:
                           tuple(ops.batch_slice(e, lo, hi) for e in enc), half_K[lo:hi])
 
     # -- steady state ---------------------------------------------------------------------------------------------------
-    def submit(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K, out=None):
+    def submit(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K, out=None,
+               reference_id=None, measurement_ids=None):
         """Buffer keyframe t (inputs CPU-pinned or CUDA): its inputs are copied now, its stages are launched when its group of
         `lookahead` keyframes is complete (or at flush() / synchronize()).  `out` as in PipelinedFusionnet.submit.
 
         The engine behaves as if it had consumed its inputs on the caller's current stream at the time of submit(): work
         the caller enqueues later on that stream may overwrite or free the CUDA inputs, and pinned host inputs may be
         rewritten once that stream has passed the submit() (e.g. after torch.cuda.current_stream().synchronize()).  At the
-        first submit() of a group that stream also waits until the group's previous use has finished."""
+        first submit() of a group that stream also waits until the group's previous use has finished.
+        Engines built with feature_cache=N take frame ids as PipelinedFusionnet.submit does; every ValueError is raised
+        before anything is copied."""
+        hits = _cache_hits(self.cache, self.M, measurement_images, reference_id, measurement_ids)
         g = self._gi % self.G
         grp = self.groups[g]
         ki = g * self.T + self._fill
         frame = (reference_image, reference_pose, measurement_images, measurement_poses, full_K)
+        ring_index = None if hits is None else _reserve_keyframe(self.cache, grp, self._fill, reference_id, measurement_ids, hits)
         # group reuse: every stage of this group's previous use has finished reading its buffers
         _take_inputs(self.kslots[ki], frame, grp["rec_done"] if self._fill == 0 else None, self.streams[0], self.streams[4],
-                     self.device, out)
+                     self.device, out, hits, ring_index)
         self._pending.append((ki, self._has_state, out, self.t))
         self._has_state = True
         self._fill += 1
@@ -821,11 +973,13 @@ class LookaheadFusionnet:
             return
         grp = self.groups[self._gi % self.G]
         s4 = self.streams[4]
-        for i, (key, body) in enumerate(_group_stages(self.mods, self.depth_args)):
+        for i, (key, body) in enumerate(_group_stages(self.mods, self.depth_args, self.cache)):
             stream = self.streams[i]
             with torch.cuda.stream(stream):
                 if i > 0:
                     stream.wait_event(grp["done"][i - 1])
+                if i == 2 and self.cache is not None:
+                    _store_misses(self.mods, self.cache, grp, self.B)
                 if grp["graph"][i] is None:
                     grp["graph"][i], grp[key], self._kernels[i] = self._capture(lambda: body(grp), stream)
                 grp["graph"][i].replay()
@@ -842,6 +996,8 @@ class LookaheadFusionnet:
                     out.copy_(ks["depth"], non_blocking=True)
                 ks["done"].record(s4)
         grp["rec_done"].record(s4)
+        if self.cache is not None:
+            self.cache.unpin()
         self.kernels_per_keyframe = sum(self._kernels[:4]) / float(self.T) + self._kernels[4]      # a full group's share + the recurrent stage
         self._pending = []
         self._fill = 0
@@ -849,11 +1005,16 @@ class LookaheadFusionnet:
 
     def prime(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K):
         """Captures every graph (both variants of the recurrent stage for the slot the next clip starts in) with
-        2 x n_groups x lookahead throw-away keyframes, then resets the clip state."""
-        for _ in range(2 * self.G * self.T):
-            self.submit(reference_image, reference_pose, measurement_images, measurement_poses, full_K)
+        2 x n_groups x lookahead throw-away keyframes, then resets the clip state (and clears the feature cache, whose
+        throw-away ids missed)."""
+        for k in range(2 * self.G * self.T):
+            self.submit(reference_image, reference_pose, measurement_images, measurement_poses, full_K,
+                        **(_prime_ids(k, self.M) if self.cache is not None else {}))
         self.synchronize()
         self.reset()
+        if self.cache is not None:
+            self.cache.clear()
+            self.cache.hits = self.cache.misses = 0
 
     def depth_of(self, t):
         """The (B,H,W) depth buffer of keyframe t, valid after synchronisation from the launch of its group (flush()) until
@@ -874,7 +1035,7 @@ class LookaheadPairnet:
     """LookaheadFusionnet's throughput engine for pairnet modules (build_modules(..., pairnet=True)).  Pairnet carries no state
     from one keyframe to the next, so the decoder runs batched over time too: every stage -- trunk head | trunk tail + feature
     pyramid | plane sweep | cost-volume encoder | decoder -- is one CUDA graph per group of `lookahead` x B keyframes, on its
-    own stream, chained by per-group events.  Every keyframe still gets all of its M + 1 feature passes (no feature cache).
+    own stream, chained by per-group events.  Without feature_cache every keyframe gets all of its M + 1 feature passes.
     Same API as LookaheadFusionnet minus load_state, so a caller can swap one for the other:
 
         eng = LookaheadPairnet(mods, batch=B, height=H, width=W, n_measurement_frames=M, lookahead=4)
@@ -882,12 +1043,15 @@ class LookaheadPairnet:
         eng.synchronize()
 
     Each batch row is computed on its own, so a keyframe's depth does not depend on its neighbours in the group; against
-    keyframe() the results differ only by the split-K choice of a few convolutions, which depends on the batch."""
+    keyframe() the results differ only by the split-K choice of a few convolutions, which depends on the batch.
+
+    feature_cache=N: the feature cache of LookaheadFusionnet(feature_cache=N), with the same frame ids at submit().
+    """
 
     n_stages = 5
 
     def __init__(self, mods, batch, height, width, n_measurement_frames, min_depth=0.25, max_depth=20.0, n_depth_levels=64,
-                 device=None, lookahead=4, n_groups=3):
+                 device=None, lookahead=4, n_groups=3, feature_cache=0):
         if "lstm" in mods:
             raise ValueError("LookaheadPairnet runs pairnet modules; fusionnet modules (with 'lstm') go to LookaheadFusionnet")
         if lookahead < 1 or n_groups < 2:
@@ -897,15 +1061,18 @@ class LookaheadPairnet:
         dev = device or next(mods["fe"].parameters()).device
         self.device = dev
         self.T, self.G = int(lookahead), int(n_groups)
+        self.cache = _lookahead_cache(feature_cache, self.T, batch, height, width, n_measurement_frames, dev)
         z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
         self.groups, self.kslots = [], []
         for g in range(self.G):
             grp = _group_buffers(self.T, batch, height, width, n_measurement_frames, dev)
+            if self.cache is not None:
+                _ring_buffers(grp, self.cache, self.T, batch, height, width, n_measurement_frames)
             grp.update({"graph": [None] * 5, "done": [torch.cuda.Event() for _ in range(5)]})
             self.groups.append(grp)
             for j in range(self.T):
                 self.kslots.append(dict(_keyframe_rows(grp, j, batch), group=g, depth=z(batch, height, width)))
-        self.stages = _pairnet_group_stages(mods, self.depth_args)
+        self.stages = _pairnet_group_stages(mods, self.depth_args, self.cache)
         # no loop-carried stage to favour: all streams at the same priority
         self.streams = [torch.cuda.Stream(device=dev) for _ in range(5)]
         self.stream_a, self.stream_b = self.streams[0], self.streams[-1]
@@ -919,7 +1086,8 @@ class LookaheadPairnet:
         """Does nothing: pairnet keyframes carry no state from one to the next, so there is no clip state to drop.  Kept so
         that code written for LookaheadFusionnet (reset() at a new clip or on tracking loss) runs unchanged."""
 
-    def submit(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K, out=None):
+    def submit(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K, out=None,
+               reference_id=None, measurement_ids=None):
         """Buffer keyframe t (inputs CPU-pinned or CUDA): its inputs are copied now, its group's stages are launched when the
         group of `lookahead` keyframes is complete (or at flush() / synchronize()).  If `out` (pinned host or CUDA tensor
         (B,H,W)) is given, the depth is copied into it on the decoder's stream; otherwise read eng.depth_of(t).
@@ -927,14 +1095,18 @@ class LookaheadPairnet:
         The engine behaves as if it had consumed its inputs on the caller's current stream at the time of submit(): work
         the caller enqueues later on that stream may overwrite or free the CUDA inputs, and pinned host inputs may be
         rewritten once that stream has passed the submit() (e.g. after torch.cuda.current_stream().synchronize()).  At the
-        first submit() of a group that stream also waits until the decoder stage of the group's previous use has finished."""
+        first submit() of a group that stream also waits until the decoder stage of the group's previous use has finished.
+        Engines built with feature_cache=N take frame ids as PipelinedFusionnet.submit does; every ValueError is raised
+        before anything is copied."""
+        hits = _cache_hits(self.cache, self.M, measurement_images, reference_id, measurement_ids)
         g = self._gi % self.G
         grp = self.groups[g]
         ki = g * self.T + self._fill
         frame = (reference_image, reference_pose, measurement_images, measurement_poses, full_K)
+        ring_index = None if hits is None else _reserve_keyframe(self.cache, grp, self._fill, reference_id, measurement_ids, hits)
         # group reuse: the decoder stage of this group's previous use ran after every other stage of that use
         _take_inputs(self.kslots[ki], frame, grp["done"][4] if self._fill == 0 else None, self.streams[0], self.streams[4],
-                     self.device, out)
+                     self.device, out, hits, ring_index)
         self._pending.append((ki, out, self.t))
         self._fill += 1
         self.t += 1
@@ -954,6 +1126,8 @@ class LookaheadPairnet:
             with torch.cuda.stream(stream):
                 if i > 0:
                     stream.wait_event(grp["done"][i - 1])
+                if i == 2 and self.cache is not None:
+                    _store_misses(self.mods, self.cache, grp, self.B)
                 if grp["graph"][i] is None:
                     torch.cuda.synchronize(self.device)
                     grp["graph"][i], grp[key], self._kernels[i] = _capture_graph(lambda: body(grp), stream, False)
@@ -967,6 +1141,8 @@ class LookaheadPairnet:
                         if out is not None:
                             out.copy_(ks["depth"], non_blocking=True)
                 grp["done"][i].record(stream)
+        if self.cache is not None:
+            self.cache.unpin()
         self.kernels_per_keyframe = sum(self._kernels) / float(self.T)      # a full group's launches per keyframe
         self._pending = []
         self._fill = 0
@@ -974,10 +1150,14 @@ class LookaheadPairnet:
 
     def prime(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K):
         """Captures every group's graphs with n_groups x lookahead throw-away keyframes, so that the one-off captures stay out
-        of a timed or latency-sensitive region."""
-        for _ in range(self.G * self.T):
-            self.submit(reference_image, reference_pose, measurement_images, measurement_poses, full_K)
+        of a timed or latency-sensitive region; then clears the feature cache, whose throw-away ids missed."""
+        for k in range(self.G * self.T):
+            self.submit(reference_image, reference_pose, measurement_images, measurement_poses, full_K,
+                        **(_prime_ids(k, self.M) if self.cache is not None else {}))
         self.synchronize()
+        if self.cache is not None:
+            self.cache.clear()
+            self.cache.hits = self.cache.misses = 0
 
     def depth_of(self, t):
         """The (B,H,W) depth buffer of keyframe t, valid after synchronisation from the launch of its group (flush()) until
