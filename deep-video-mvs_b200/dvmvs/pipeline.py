@@ -363,6 +363,11 @@ def _cache_hits(cache, M, measurement_images, reference_id, measurement_ids):
     return hits
 
 
+def _prime_ids(k, M):
+    """Throw-away frame ids of prime()'s k-th keyframe: all misses, so that the miss path is exercised too."""
+    return {"reference_id": ("prime", k), "measurement_ids": [("prime-m", k, m) for m in range(M)]}
+
+
 def _load_state(self, lstm_state, previous_depth, previous_pose):
     """Continue a clip whose first keyframes ran elsewhere (e.g. through the module calls with fewer measurement frames):
     installs (h, c), the previous depth (B,1,H,W) and the previous pose as the recurrent state of the next submit().
@@ -675,11 +680,8 @@ class PipelinedFusionnet:
         keyframes, then resets the clip state.  Optional: submit() captures lazily; call this to keep the one-off
         captures out of a timed or latency-sensitive region."""
         for k in range(2 * self.n_stages):
-            if self.cache is not None:
-                self.submit(reference_image, reference_pose, measurement_images, measurement_poses, full_K,
-                            reference_id=("prime", k), measurement_ids=[("prime-m", k, m) for m in range(self.M)])
-            else:
-                self.submit(reference_image, reference_pose, measurement_images, measurement_poses, full_K)
+            self.submit(reference_image, reference_pose, measurement_images, measurement_poses, full_K,
+                        **(_prime_ids(k, self.M) if self.cache is not None else {}))
         self.synchronize()
         self.reset()
         if self.cache is not None:
@@ -836,12 +838,152 @@ def _lookahead_cache(feature_cache, T, B, H, W, M, device):
     return cache
 
 
-def _prime_ids(k, M):
-    """Throw-away frame ids of prime()'s k-th keyframe: all misses, so that the miss path is exercised too."""
-    return {"reference_id": ("prime", k), "measurement_ids": [("prime-m", k, m) for m in range(M)]}
+class _LookaheadEngine:
+    """What LookaheadFusionnet and LookaheadPairnet share.  submit() buffers keyframes into the open group of `lookahead`
+    keyframes; flush() launches it: each of the engine's group stages (self.stages, (key, body) pairs) is one CUDA graph per
+    group on its own stream, chained by the group's `done` events (done[i]: stream i has run its part of the group), then on
+    the last stream, for each buffered keyframe in order, the engine's _keyframe_stage and the copy of the keyframe's depth
+    into `out`.  done[4], recorded after that, is what the group's next first submit() waits for.  `kslots` hold each keyframe's rows of its
+    group's inputs, its depth buffer and the graphs of its per-keyframe stage (none for pairnet)."""
+
+    n_stages = 5
+    _prime_rounds = 1                     # prime() submits _prime_rounds x n_groups x lookahead throw-away keyframes
+
+    def __init__(self, stages, mods, batch, height, width, n_measurement_frames, min_depth, max_depth, n_depth_levels, device,
+                 lookahead, n_groups, feature_cache, last_priority=0):
+        """stages(mods, depth_args, cache): the engine's group stages.  last_priority: the last stream's priority."""
+        if lookahead < 1 or n_groups < 2:
+            raise ValueError("lookahead >= 1 and n_groups >= 2 required")
+        self.mods, self.B, self.H, self.W, self.M = mods, batch, height, width, n_measurement_frames
+        self.depth_args = (min_depth, max_depth, n_depth_levels)
+        dev = device or next(mods["fe"].parameters()).device
+        self.device = dev
+        self.T, self.G = int(lookahead), int(n_groups)
+        self.cache = _lookahead_cache(feature_cache, self.T, batch, height, width, n_measurement_frames, dev)
+        self.stages = stages(mods, self.depth_args, self.cache)
+        n = len(self.stages)
+        self.groups, self.kslots = [], []
+        for _ in range(self.G):
+            grp = _group_buffers(self.T, batch, height, width, n_measurement_frames, dev)
+            if self.cache is not None:
+                _ring_buffers(grp, self.cache, self.T, batch, height, width, n_measurement_frames)
+            grp.update({"graph": [None] * n, "done": [torch.cuda.Event() for _ in range(5)]})
+            self.groups.append(grp)
+            for j in range(self.T):
+                self.kslots.append(dict(_keyframe_rows(grp, j, batch), graph=dict(),
+                                        depth=torch.zeros(batch, height, width, dtype=torch.float32, device=dev)))
+        self.streams = [torch.cuda.Stream(device=dev, priority=(last_priority if i == 4 else 0)) for i in range(5)]
+        self.stream_a, self.stream_b = self.streams[0], self.streams[-1]
+        self._has_state = False              # the next submitted keyframe continues a clip (read by the recurrent stage only)
+        self._gi, self._fill = 0, 0          # group counter, keyframes buffered in the open group
+        self._pending = []                   # (kslot index, with_state, out, t) of the open group
+        self.t = 0
+        self._kernels = [0] * 5
+        self.kernels_per_keyframe = 0
+
+    def _capture(self, fn, stream, pdl=False, *state):
+        """_capture_graph on an otherwise idle device.  No PDL by default: it costs throughput with stages in flight (see
+        PipelinedFusionnet)."""
+        torch.cuda.synchronize(self.device)
+        captured = _capture_graph(fn, stream, pdl, *state)
+        torch.cuda.synchronize(self.device)
+        return captured
+
+    # -- steady state ---------------------------------------------------------------------------------------------------
+    def submit(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K, out=None,
+               reference_id=None, measurement_ids=None):
+        """Buffer keyframe t (inputs CPU-pinned or CUDA): its inputs are copied now, its group's stages are launched when the
+        group of `lookahead` keyframes is complete (or at flush() / synchronize()).  If `out` (pinned host or CUDA tensor
+        (B,H,W)) is given, the depth is copied into it on the last stream; otherwise read eng.depth_of(t).
+
+        The engine behaves as if it had consumed its inputs on the caller's current stream at the time of submit(): work
+        the caller enqueues later on that stream may overwrite or free the CUDA inputs, and pinned host inputs may be
+        rewritten once that stream has passed the submit() (e.g. after torch.cuda.current_stream().synchronize()).  At the
+        first submit() of a group that stream also waits until the group's previous use has finished.
+        Engines built with feature_cache=N take frame ids as PipelinedFusionnet.submit does; every ValueError is raised
+        before anything is copied."""
+        hits = _cache_hits(self.cache, self.M, measurement_images, reference_id, measurement_ids)
+        g = self._gi % self.G
+        grp = self.groups[g]
+        ki = g * self.T + self._fill
+        frame = (reference_image, reference_pose, measurement_images, measurement_poses, full_K)
+        ring_index = None if hits is None else _reserve_keyframe(self.cache, grp, self._fill, reference_id, measurement_ids, hits)
+        # group reuse: all work of this group's previous use has finished reading its buffers
+        _take_inputs(self.kslots[ki], frame, grp["done"][4] if self._fill == 0 else None, self.streams[0], self.streams[4],
+                     self.device, out, hits, ring_index)
+        self._pending.append((ki, self._has_state, out, self.t))
+        self._has_state = True
+        self._fill += 1
+        self.t += 1
+        if self._fill == self.T:
+            self.flush()
+        return self.t - 1
+
+    def flush(self):
+        """Launch the open group (complete or not): stream i runs group stage i, if the engine has one, over the group's
+        buffers; the last stream then runs each buffered keyframe's per-keyframe stage and the copy of its depth into `out`,
+        in order.  Rows no keyframe filled keep the finite inputs they held before; their results are not read.  Each stream
+        is entered once and records one event: at small sizes the host's enqueue cost bounds the engine's rate."""
+        if not self._pending:
+            return
+        grp = self.groups[self._gi % self.G]
+        for i, stream in enumerate(self.streams):
+            with torch.cuda.stream(stream):
+                if i < len(self.stages):
+                    key, body = self.stages[i]
+                    if i > 0:
+                        stream.wait_event(grp["done"][i - 1])
+                    if i == 2 and self.cache is not None:
+                        _store_misses(self.mods, self.cache, grp, self.B)
+                    if grp["graph"][i] is None:
+                        grp["graph"][i], grp[key], self._kernels[i] = self._capture(lambda: body(grp), stream)
+                    grp["graph"][i].replay()
+                if i == 4:
+                    for ki, with_state, out, t in self._pending:
+                        ks = self.kslots[ki]
+                        ks["t"] = t
+                        self._keyframe_stage(ks, grp, with_state)
+                        if out is not None:
+                            out.copy_(ks["depth"], non_blocking=True)
+                grp["done"][i].record(stream)
+        if self.cache is not None:
+            self.cache.unpin()
+        n = len(self.stages)          # a full group's share of the group stages' launches + the per-keyframe stage's
+        self.kernels_per_keyframe = sum(self._kernels[:n]) / float(self.T) + sum(self._kernels[n:])
+        self._pending = []
+        self._fill = 0
+        self._gi += 1
+
+    def prime(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K):
+        """Captures every graph with throw-away keyframes (LookaheadFusionnet: 2 x n_groups x lookahead, so that the slot the
+        next clip starts in has both variants of its recurrent stage; LookaheadPairnet: n_groups x lookahead), so that the
+        one-off captures stay out of a timed or latency-sensitive region; then resets the clip state and clears the feature
+        cache, whose throw-away ids missed."""
+        for k in range(self._prime_rounds * self.G * self.T):
+            self.submit(reference_image, reference_pose, measurement_images, measurement_poses, full_K,
+                        **(_prime_ids(k, self.M) if self.cache is not None else {}))
+        self.synchronize()
+        self.reset()
+        if self.cache is not None:
+            self.cache.clear()
+            self.cache.hits = self.cache.misses = 0
+
+    def depth_of(self, t):
+        """The (B,H,W) depth buffer of keyframe t, valid after synchronisation from the launch of its group (flush()) until
+        the launch of the next keyframe in its slot.  Raises KeyError for a t no slot holds: stale, not yet submitted, or
+        buffered in a group not launched yet."""
+        for ks in self.kslots:
+            if ks.get("t") == t:
+                return ks["depth"]
+        raise KeyError("keyframe %r: no keyframe slot holds its depth" % (t,))
+
+    def synchronize(self):
+        self.flush()
+        for s in self.streams:
+            s.synchronize()
 
 
-class LookaheadFusionnet:
+class LookaheadFusionnet(_LookaheadEngine):
     """Throughput engine with everything that does NOT depend on the recurrent state batched over TIME: FeatureExtractor,
     FeatureShrinker, the plane sweep and the cost-volume encoder run once per group of `lookahead` consecutive keyframes
     (lookahead x B "clips", each with its own poses and its own M measurement frames) instead of once per keyframe; only the
@@ -871,45 +1013,19 @@ class LookaheadFusionnet:
         eng.synchronize()
     """
 
-    n_stages = 5
+    _prime_rounds = 2
 
     def __init__(self, mods, batch, height, width, n_measurement_frames, min_depth=0.25, max_depth=20.0, n_depth_levels=64,
                  device=None, lookahead=4, n_groups=3, feature_cache=0):
-        if lookahead < 1 or n_groups < 2:
-            raise ValueError("lookahead >= 1 and n_groups >= 2 required")
-        self.mods, self.B, self.H, self.W, self.M = mods, batch, height, width, n_measurement_frames
-        self.depth_args = (min_depth, max_depth, n_depth_levels)
-        dev = device or next(mods["fe"].parameters()).device
-        self.device = dev
-        self.T, self.G = int(lookahead), int(n_groups)
-        self.cache = _lookahead_cache(feature_cache, self.T, batch, height, width, n_measurement_frames, dev)
-        z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
-        self.groups, self.kslots = [], []
-        for g in range(self.G):
-            grp = _group_buffers(self.T, batch, height, width, n_measurement_frames, dev)
-            if self.cache is not None:
-                _ring_buffers(grp, self.cache, self.T, batch, height, width, n_measurement_frames)
-            grp.update({"head": None, "pyramid": None, "swept": None, "enc": None, "graph": [None] * 4,
-                        "done": [torch.cuda.Event() for _ in range(4)], "rec_done": torch.cuda.Event()})
-            self.groups.append(grp)
-            for j in range(self.T):
-                self.kslots.append(dict(_keyframe_rows(grp, j, batch), group=g, depth=z(batch, height, width), graph=dict(),
-                                        done=torch.cuda.Event()))
         # the recurrent stage's small kernels carry the loop dependence; on a high-priority stream their CTAs are dispatched
         # ahead of the queued CTAs of the batched stages' big grids (DVMVS_LA_PRIO=0: all streams equal)
         prio = os.environ.get("DVMVS_LA_PRIO", "1") == "1"
+        super().__init__(_group_stages, mods, batch, height, width, n_measurement_frames, min_depth, max_depth, n_depth_levels,
+                         device, lookahead, n_groups, feature_cache, last_priority=(-1 if prio else 0))
         # experiment switch, off: DVMVS_LA_REC_PDL=1 captures the recurrent stage's graph with programmatic dependent launch
         # (measured slower, as for the other stages)
         self._rec_pdl = os.environ.get("DVMVS_LA_REC_PDL", "0") == "1"
-        self.streams = [torch.cuda.Stream(device=dev, priority=(-1 if (prio and i == 4) else 0)) for i in range(5)]
-        self.stream_a, self.stream_b = self.streams[0], self.streams[-1]
         self._static_state = _StaticState()
-        self._has_state = False
-        self._gi, self._fill = 0, 0          # group counter, keyframes buffered in the open group
-        self._pending = []                   # (kslot index, with_state, out, t) of the open group
-        self.t = 0
-        self._kernels = [0] * 5
-        self.kernels_per_keyframe = 0
 
     def reset(self):
         """New clip / tracking lost: the next submitted keyframe starts without recurrent state (buffered keyframes keep theirs).
@@ -917,15 +1033,6 @@ class LookaheadFusionnet:
         self._has_state = False
 
     load_state = _load_state
-
-    def _capture(self, fn, stream, ks=None):
-        """Graph of one of a group's batched stages, or (`ks`) of the recurrent stage of keyframe slot `ks`; returns what
-        _capture_graph returns.  No PDL: it costs throughput with stages in flight (see PipelinedFusionnet)."""
-        torch.cuda.synchronize(self.device)
-        captured = _capture_graph(fn, stream, ks is not None and self._rec_pdl,
-                                  *((self._static_state, ks["depth"]) if ks is not None else ()))
-        torch.cuda.synchronize(self.device)
-        return captured
 
     def _run_rec(self, ks, grp, with_state):
         lo, hi = ks["lo"], ks["hi"]
@@ -937,101 +1044,17 @@ class LookaheadFusionnet:
         return _stage_rec(self.mods, self._static_state.keyframe_state(with_state), view,
                           tuple(ops.batch_slice(e, lo, hi) for e in enc), half_K[lo:hi])
 
-    # -- steady state ---------------------------------------------------------------------------------------------------
-    def submit(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K, out=None,
-               reference_id=None, measurement_ids=None):
-        """Buffer keyframe t (inputs CPU-pinned or CUDA): its inputs are copied now, its stages are launched when its group of
-        `lookahead` keyframes is complete (or at flush() / synchronize()).  `out` as in PipelinedFusionnet.submit.
-
-        The engine behaves as if it had consumed its inputs on the caller's current stream at the time of submit(): work
-        the caller enqueues later on that stream may overwrite or free the CUDA inputs, and pinned host inputs may be
-        rewritten once that stream has passed the submit() (e.g. after torch.cuda.current_stream().synchronize()).  At the
-        first submit() of a group that stream also waits until the group's previous use has finished.
-        Engines built with feature_cache=N take frame ids as PipelinedFusionnet.submit does; every ValueError is raised
-        before anything is copied."""
-        hits = _cache_hits(self.cache, self.M, measurement_images, reference_id, measurement_ids)
-        g = self._gi % self.G
-        grp = self.groups[g]
-        ki = g * self.T + self._fill
-        frame = (reference_image, reference_pose, measurement_images, measurement_poses, full_K)
-        ring_index = None if hits is None else _reserve_keyframe(self.cache, grp, self._fill, reference_id, measurement_ids, hits)
-        # group reuse: every stage of this group's previous use has finished reading its buffers
-        _take_inputs(self.kslots[ki], frame, grp["rec_done"] if self._fill == 0 else None, self.streams[0], self.streams[4],
-                     self.device, out, hits, ring_index)
-        self._pending.append((ki, self._has_state, out, self.t))
-        self._has_state = True
-        self._fill += 1
-        self.t += 1
-        if self._fill == self.T:
-            self.flush()
-        return self.t - 1
-
-    def flush(self):
-        """Launch the open group (complete or not): trunk, pyramid, plane sweep and encoder over the group's buffers, then the
-        recurrent stage for each buffered keyframe in order."""
-        if not self._pending:
-            return
-        grp = self.groups[self._gi % self.G]
+    def _keyframe_stage(self, ks, grp, with_state):
+        """The recurrent stage of keyframe slot `ks` (its graph with or without state), after the group's encoder."""
         s4 = self.streams[4]
-        for i, (key, body) in enumerate(_group_stages(self.mods, self.depth_args, self.cache)):
-            stream = self.streams[i]
-            with torch.cuda.stream(stream):
-                if i > 0:
-                    stream.wait_event(grp["done"][i - 1])
-                if i == 2 and self.cache is not None:
-                    _store_misses(self.mods, self.cache, grp, self.B)
-                if grp["graph"][i] is None:
-                    grp["graph"][i], grp[key], self._kernels[i] = self._capture(lambda: body(grp), stream)
-                grp["graph"][i].replay()
-                grp["done"][i].record(stream)
-        for ki, with_state, out, t in self._pending:
-            ks = self.kslots[ki]
-            ks["t"] = t
-            with torch.cuda.stream(s4):
-                s4.wait_event(grp["done"][3])
-                if with_state not in ks["graph"]:
-                    ks["graph"][with_state], _, self._kernels[4] = self._capture(lambda: self._run_rec(ks, grp, with_state), s4, ks)
-                ks["graph"][with_state].replay()
-                if out is not None:
-                    out.copy_(ks["depth"], non_blocking=True)
-                ks["done"].record(s4)
-        grp["rec_done"].record(s4)
-        if self.cache is not None:
-            self.cache.unpin()
-        self.kernels_per_keyframe = sum(self._kernels[:4]) / float(self.T) + self._kernels[4]      # a full group's share + the recurrent stage
-        self._pending = []
-        self._fill = 0
-        self._gi += 1
-
-    def prime(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K):
-        """Captures every graph (both variants of the recurrent stage for the slot the next clip starts in) with
-        2 x n_groups x lookahead throw-away keyframes, then resets the clip state (and clears the feature cache, whose
-        throw-away ids missed)."""
-        for k in range(2 * self.G * self.T):
-            self.submit(reference_image, reference_pose, measurement_images, measurement_poses, full_K,
-                        **(_prime_ids(k, self.M) if self.cache is not None else {}))
-        self.synchronize()
-        self.reset()
-        if self.cache is not None:
-            self.cache.clear()
-            self.cache.hits = self.cache.misses = 0
-
-    def depth_of(self, t):
-        """The (B,H,W) depth buffer of keyframe t, valid after synchronisation from the launch of its group (flush()) until
-        the launch of the next keyframe in its slot.  Raises KeyError for a t no slot holds: stale, not yet submitted, or
-        buffered in a group not launched yet."""
-        for ks in self.kslots:
-            if ks.get("t") == t:
-                return ks["depth"]
-        raise KeyError("keyframe %r: no keyframe slot holds its depth" % (t,))
-
-    def synchronize(self):
-        self.flush()
-        for s in self.streams:
-            s.synchronize()
+        s4.wait_event(grp["done"][3])
+        if with_state not in ks["graph"]:
+            ks["graph"][with_state], _, self._kernels[4] = self._capture(lambda: self._run_rec(ks, grp, with_state), s4,
+                                                                         self._rec_pdl, self._static_state, ks["depth"])
+        ks["graph"][with_state].replay()
 
 
-class LookaheadPairnet:
+class LookaheadPairnet(_LookaheadEngine):
     """LookaheadFusionnet's throughput engine for pairnet modules (build_modules(..., pairnet=True)).  Pairnet carries no state
     from one keyframe to the next, so the decoder runs batched over time too: every stage -- trunk head | trunk tail + feature
     pyramid | plane sweep | cost-volume encoder | decoder -- is one CUDA graph per group of `lookahead` x B keyframes, on its
@@ -1048,130 +1071,21 @@ class LookaheadPairnet:
     feature_cache=N: the feature cache of LookaheadFusionnet(feature_cache=N), with the same frame ids at submit().
     """
 
-    n_stages = 5
-
     def __init__(self, mods, batch, height, width, n_measurement_frames, min_depth=0.25, max_depth=20.0, n_depth_levels=64,
                  device=None, lookahead=4, n_groups=3, feature_cache=0):
         if "lstm" in mods:
             raise ValueError("LookaheadPairnet runs pairnet modules; fusionnet modules (with 'lstm') go to LookaheadFusionnet")
-        if lookahead < 1 or n_groups < 2:
-            raise ValueError("lookahead >= 1 and n_groups >= 2 required")
-        self.mods, self.B, self.H, self.W, self.M = mods, batch, height, width, n_measurement_frames
-        self.depth_args = (min_depth, max_depth, n_depth_levels)
-        dev = device or next(mods["fe"].parameters()).device
-        self.device = dev
-        self.T, self.G = int(lookahead), int(n_groups)
-        self.cache = _lookahead_cache(feature_cache, self.T, batch, height, width, n_measurement_frames, dev)
-        z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=dev)
-        self.groups, self.kslots = [], []
-        for g in range(self.G):
-            grp = _group_buffers(self.T, batch, height, width, n_measurement_frames, dev)
-            if self.cache is not None:
-                _ring_buffers(grp, self.cache, self.T, batch, height, width, n_measurement_frames)
-            grp.update({"graph": [None] * 5, "done": [torch.cuda.Event() for _ in range(5)]})
-            self.groups.append(grp)
-            for j in range(self.T):
-                self.kslots.append(dict(_keyframe_rows(grp, j, batch), group=g, depth=z(batch, height, width)))
-        self.stages = _pairnet_group_stages(mods, self.depth_args, self.cache)
         # no loop-carried stage to favour: all streams at the same priority
-        self.streams = [torch.cuda.Stream(device=dev) for _ in range(5)]
-        self.stream_a, self.stream_b = self.streams[0], self.streams[-1]
-        self._gi, self._fill = 0, 0          # group counter, keyframes buffered in the open group
-        self._pending = []                   # (kslot index, out, t) of the open group
-        self.t = 0
-        self._kernels = [0] * 5
-        self.kernels_per_keyframe = 0
+        super().__init__(_pairnet_group_stages, mods, batch, height, width, n_measurement_frames, min_depth, max_depth,
+                         n_depth_levels, device, lookahead, n_groups, feature_cache)
 
     def reset(self):
         """Does nothing: pairnet keyframes carry no state from one to the next, so there is no clip state to drop.  Kept so
         that code written for LookaheadFusionnet (reset() at a new clip or on tracking loss) runs unchanged."""
 
-    def submit(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K, out=None,
-               reference_id=None, measurement_ids=None):
-        """Buffer keyframe t (inputs CPU-pinned or CUDA): its inputs are copied now, its group's stages are launched when the
-        group of `lookahead` keyframes is complete (or at flush() / synchronize()).  If `out` (pinned host or CUDA tensor
-        (B,H,W)) is given, the depth is copied into it on the decoder's stream; otherwise read eng.depth_of(t).
-
-        The engine behaves as if it had consumed its inputs on the caller's current stream at the time of submit(): work
-        the caller enqueues later on that stream may overwrite or free the CUDA inputs, and pinned host inputs may be
-        rewritten once that stream has passed the submit() (e.g. after torch.cuda.current_stream().synchronize()).  At the
-        first submit() of a group that stream also waits until the decoder stage of the group's previous use has finished.
-        Engines built with feature_cache=N take frame ids as PipelinedFusionnet.submit does; every ValueError is raised
-        before anything is copied."""
-        hits = _cache_hits(self.cache, self.M, measurement_images, reference_id, measurement_ids)
-        g = self._gi % self.G
-        grp = self.groups[g]
-        ki = g * self.T + self._fill
-        frame = (reference_image, reference_pose, measurement_images, measurement_poses, full_K)
-        ring_index = None if hits is None else _reserve_keyframe(self.cache, grp, self._fill, reference_id, measurement_ids, hits)
-        # group reuse: the decoder stage of this group's previous use ran after every other stage of that use
-        _take_inputs(self.kslots[ki], frame, grp["done"][4] if self._fill == 0 else None, self.streams[0], self.streams[4],
-                     self.device, out, hits, ring_index)
-        self._pending.append((ki, out, self.t))
-        self._fill += 1
-        self.t += 1
-        if self._fill == self.T:
-            self.flush()
-        return self.t - 1
-
-    def flush(self):
-        """Launch the open group (complete or not): the five stages over the group's buffers, then each buffered keyframe's
-        rows of the group's depth copied into its own depth buffer (and `out`).  Rows no keyframe filled keep the finite
-        inputs they held before; their results are not read."""
-        if not self._pending:
-            return
-        grp = self.groups[self._gi % self.G]
-        for i, (key, body) in enumerate(self.stages):
-            stream = self.streams[i]
-            with torch.cuda.stream(stream):
-                if i > 0:
-                    stream.wait_event(grp["done"][i - 1])
-                if i == 2 and self.cache is not None:
-                    _store_misses(self.mods, self.cache, grp, self.B)
-                if grp["graph"][i] is None:
-                    torch.cuda.synchronize(self.device)
-                    grp["graph"][i], grp[key], self._kernels[i] = _capture_graph(lambda: body(grp), stream, False)
-                    torch.cuda.synchronize(self.device)
-                grp["graph"][i].replay()
-                if i == 4:
-                    for ki, out, t in self._pending:
-                        ks = self.kslots[ki]
-                        ks["t"] = t
-                        ks["depth"].copy_(grp["depth"][ks["lo"]:ks["hi"]], non_blocking=True)
-                        if out is not None:
-                            out.copy_(ks["depth"], non_blocking=True)
-                grp["done"][i].record(stream)
-        if self.cache is not None:
-            self.cache.unpin()
-        self.kernels_per_keyframe = sum(self._kernels) / float(self.T)      # a full group's launches per keyframe
-        self._pending = []
-        self._fill = 0
-        self._gi += 1
-
-    def prime(self, reference_image, reference_pose, measurement_images, measurement_poses, full_K):
-        """Captures every group's graphs with n_groups x lookahead throw-away keyframes, so that the one-off captures stay out
-        of a timed or latency-sensitive region; then clears the feature cache, whose throw-away ids missed."""
-        for k in range(self.G * self.T):
-            self.submit(reference_image, reference_pose, measurement_images, measurement_poses, full_K,
-                        **(_prime_ids(k, self.M) if self.cache is not None else {}))
-        self.synchronize()
-        if self.cache is not None:
-            self.cache.clear()
-            self.cache.hits = self.cache.misses = 0
-
-    def depth_of(self, t):
-        """The (B,H,W) depth buffer of keyframe t, valid after synchronisation from the launch of its group (flush()) until
-        the launch of the next keyframe in its slot.  Raises KeyError for a t no slot holds: stale, not yet submitted, or
-        buffered in a group not launched yet."""
-        for ks in self.kslots:
-            if ks.get("t") == t:
-                return ks["depth"]
-        raise KeyError("keyframe %r: no keyframe slot holds its depth" % (t,))
-
-    def synchronize(self):
-        self.flush()
-        for s in self.streams:
-            s.synchronize()
+    def _keyframe_stage(self, ks, grp, with_state):
+        """Keyframe slot `ks`'s rows of the group's depth, after the decoder's graph on the same stream."""
+        ks["depth"].copy_(grp["depth"][ks["lo"]:ks["hi"]], non_blocking=True)
 
 
 class OnlineFusionnet:

@@ -316,8 +316,8 @@ def skips(monkeypatch):
 def _stage_graphs(eng):
     """(graph, stream) of every captured stage graph of an engine."""
     from dvmvs import pipeline
-    if isinstance(eng, pipeline.LookaheadFusionnet):
-        out = [(g["graph"][i], eng.streams[i]) for g in eng.groups for i in range(4) if g["graph"][i] is not None]
+    if isinstance(eng, (pipeline.LookaheadFusionnet, pipeline.LookaheadPairnet)):
+        out = [(gr, eng.streams[i]) for g in eng.groups for i, gr in enumerate(g["graph"]) if gr is not None]
         return out + [(gr, eng.streams[4]) for ks in eng.kslots for gr in ks["graph"].values()]
     if isinstance(eng, pipeline.PipelinedFusionnet):
         return [(gr, eng.streams[i]) for slot in eng.slots for i, d in enumerate(slot["graph"]) for gr in d.values()]
@@ -491,7 +491,7 @@ def _defects(eng, kind):
     s = eng.streams
     if kind == "lookahead":
         return [("the recurrent stream does not wait for done[3]", dict(on=s[4], events=[g["done"][3] for g in eng.groups]), [s[3]], False),
-                ("the group-reuse wait on rec_done is skipped", dict(on=None, events=[g["rec_done"] for g in eng.groups]), [s[4]], False),
+                ("the group-reuse wait on done[4] is skipped", dict(on=None, events=[g["done"][4] for g in eng.groups]), [s[4]], False),
                 ("stage 2 does not wait for done[1]", dict(on=s[2], events=[g["done"][1] for g in eng.groups]), [s[1]], False),
                 ("stream 0 does not wait for the caller's stream", dict(on=s[0], other=torch.cuda.current_stream()), [], True)]
     last = eng.n_stages - 1

@@ -14,7 +14,7 @@ import pytest
 import torch
 
 from tests import helpers, scene_fixture
-from tests.test_engine_ordering import (NAN, _Delay, _assert_same, _diff, _elapsed_ms, _frames, _lookahead_script, _map, _tc,
+from tests.test_engine_ordering import (NAN, _Delay, _assert_same, _calibrate, _diff, _frames, _lookahead_script, _map, _tc,
                                         _variants)
 
 pytestmark = pytest.mark.gpu
@@ -234,23 +234,6 @@ def _jumpy(k):
     """Keyframe index of script step k: pairs of consecutive keyframes two apart, so that every pair starts with M misses and
     each group takes more ring entries than the smallest ring keeps free -- it evicts entries the previous group reads."""
     return k + 2 * (k // 2)
-
-
-def _calibrate(eng, label):
-    torch.cuda.synchronize()
-    graphs = [(g["graph"][i], eng.streams[i]) for g in eng.groups for i in range(len(g["graph"])) if g["graph"][i] is not None]
-    graphs += [(gr, eng.streams[4]) for ks in eng.kslots for gr in ks.get("graph", {}).values()]
-    longest = max(_elapsed_ms(s, g.replay) for g, s in graphs)
-    side = torch.cuda.Stream()
-    cycles = 2_000_000
-    for _ in range(4):
-        sleep = _elapsed_ms(side, lambda: torch.cuda._sleep(cycles), reps=1)
-        if sleep >= 6.0 * longest:
-            break
-        cycles = int(cycles * 6.6 * longest / sleep) + 1
-    print("%s: %d graphs, longest replay %.3f ms; sleep of %d cycles %.3f ms" % (label, len(graphs), longest, cycles, sleep))
-    assert sleep >= 5.0 * longest
-    return cycles
 
 
 def _late_feed(feed, cycles):

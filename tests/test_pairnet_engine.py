@@ -12,8 +12,8 @@ import pytest
 import torch
 
 from tests import helpers, scene_fixture
-from tests.test_engine_ordering import (NAN, _Delay, _Skips, _assert_same, _diff, _elapsed_ms, _frames, _late, _lookahead_script,
-                                        _map, _run, _tc, _tensors, _under_delays)
+from tests.test_engine_ordering import (NAN, _Delay, _Skips, _assert_same, _calibrate, _diff, _frames, _late, _lookahead_script,
+                                        _map, _run, _stage_graphs, _tc, _tensors, _under_delays)
 
 pytestmark = pytest.mark.gpu
 
@@ -71,26 +71,6 @@ def _replay(mods, frames, script, T, B, H, W, M, D):
             flush()
     torch.cuda.synchronize()
     return depths
-
-
-def _calibrate(eng, label):
-    """Sleep cycles worth at least 5x the longest stage-graph replay of `eng` (each replayed alone, median of 3), as
-    test_engine_ordering._calibrate does for the fusionnet engines."""
-    torch.cuda.synchronize()
-    graphs = [(g["graph"][i], eng.streams[i]) for g in eng.groups for i in range(5) if g["graph"][i] is not None]
-    assert len(graphs) == 5 * eng.G
-    longest = max(_elapsed_ms(s, g.replay) for g, s in graphs)
-    side = torch.cuda.Stream()
-    cycles = 2_000_000
-    for _ in range(4):
-        sleep = _elapsed_ms(side, lambda: torch.cuda._sleep(cycles), reps=1)
-        if sleep >= 6.0 * longest:
-            break
-        cycles = int(cycles * 6.6 * longest / sleep) + 1
-    print("%s: %d stage graphs, longest replay %.3f ms; sleep of %d cycles %.3f ms (%.1fx)"
-          % (label, len(graphs), longest, cycles, sleep, sleep / longest))
-    assert sleep >= 5.0 * longest, "sleep %.3f ms is not 5x the longest stage replay %.3f ms" % (sleep, longest)
-    return cycles
 
 
 def _clip_args(clip, k):
@@ -250,6 +230,7 @@ def test_pairnet_engine_equals_its_schedule_replay_under_delayed_streams(oracle,
         ref = _replay(mods, frames, script, T, B, H, W, M, D)
         assert B == 1 or not torch.equal(ref[-1][0], ref[-1][-1]), "the batch rows hold the same clip"
         _assert_same(_run(eng, frames, script), ref, "undelayed")
+        assert len(_stage_graphs(eng)) == 5 * eng.G
         cycles = _calibrate(eng, "pairnet lookahead %s" % (cfg,))
         delay.install()
         _under_delays(eng, frames, script, ref, delay, cycles, "pairnet lookahead %s" % (cfg,))
@@ -268,6 +249,7 @@ def test_planted_ordering_defects_change_the_delayed_run(oracle, synth, delay, s
         eng.prime(*frames[0])
         ref = _replay(mods, frames, script, T, 1, H, W, M, D)
         _assert_same(_run(eng, frames, script), ref, "undelayed, no defect")
+        assert len(_stage_graphs(eng)) == 5 * eng.G
         cycles = _calibrate(eng, "pairnet defects")
         delay.install()
         s = eng.streams
@@ -335,6 +317,7 @@ def test_submit_consumes_inputs_on_the_callers_stream(oracle, synth, delay):
         eng.prime(*frames[0])
         ref = _replay(mods, frames, script, T, 1, H, W, M, D)
         _assert_same(_run(eng, frames, script), ref, "undelayed")
+        assert len(_stage_graphs(eng)) == 5 * eng.G
         cycles = _calibrate(eng, "pairnet contract")
         delay.install()
         first, last = eng.streams[:1], eng.streams[-1:]
