@@ -24,7 +24,8 @@ def sources():
 
 def _stamp():
     h = hashlib.sha256()
-    for f in sorted(os.listdir(CSRC)) + ["../../include/dvmvs_b200.h"]:
+    headers = ["../../include/" + f for f in sorted(os.listdir(os.path.join(HERE, "..", "include")))]
+    for f in sorted(os.listdir(CSRC)) + headers:
         with open(os.path.join(CSRC, f), "rb") as fh:
             h.update(f.encode() + b"\0" + fh.read())
     h.update(" ".join(FLAGS).encode())

@@ -26,6 +26,12 @@ EXPORTED_SYMBOLS = [
     "dvmvs_depth_loss_backward", "dvmvs_plane_sweep_fused_h16", "dvmvs_plane_sweep_tc", "dvmvs_lstm_gates_parts", "dvmvs_conv2d_tc_ksplit", "dvmvs_plane_sweep_tc_set_timeline",
     "dvmvs_mesh_scratch_bytes", "dvmvs_mesh_count", "dvmvs_mesh_extract", "dvmvs_tsdf_raycast",
 ]
+# every symbol include/dvmvs_tsdf_sparse.h declares (the voxel-block TSDF volume; tests/test_tsdf_sparse.py covers them)
+SPARSE_SYMBOLS = [
+    "dvmvs_tsdf_sparse_scratch_bytes", "dvmvs_tsdf_sparse_allocate", "dvmvs_tsdf_sparse_integrate", "dvmvs_tsdf_sparse_export",
+    "dvmvs_tsdf_sparse_block_bounds",
+]
+SPARSE_POOL_FULL, SPARSE_TABLE_FULL, SPARSE_FRUSTUM = 1, 2, 4
 
 
 class ConvDesc(ctypes.Structure):
@@ -138,6 +144,13 @@ def lib():
         L.dvmvs_mesh_count.argtypes = [p, i, i, i, p, ll, p]
         L.dvmvs_mesh_extract.argtypes = [p, p, i, i, i, ctypes.POINTER(ctypes.c_float), f, p, ll, i, i, p, p, p, p, p, p]
         L.dvmvs_tsdf_raycast.argtypes = [p, p, i, i, i, ctypes.POINTER(ctypes.c_float), d, d, p, i, i, i, p, p, p, p]
+        L.dvmvs_tsdf_sparse_scratch_bytes.argtypes = [i, i, ctypes.POINTER(ll)]
+        L.dvmvs_tsdf_sparse_allocate.argtypes = [p, p, i, p, i, p, p, p, ll, ctypes.POINTER(ctypes.c_float), d, d, p, i, i, i,
+                                                 ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_double), p]
+        L.dvmvs_tsdf_sparse_integrate.argtypes = [p, p, p, p, i, p, p, ctypes.POINTER(ctypes.c_float), d, d, p, i, p, i, i, i,
+                                                  ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_double), d, p, p]
+        L.dvmvs_tsdf_sparse_export.argtypes = [p, p, p, p, i, p, ctypes.POINTER(ctypes.c_int), i, i, i, p, p, p, p]
+        L.dvmvs_tsdf_sparse_block_bounds.argtypes = [p, i, p, p, p]
         L.dvmvs_plane_sweep_backward.argtypes = [p, p, p, p, p, p, p, p, i, i, i, i, i, i, f, f, i, p]
         L.dvmvs_hidden_warp_backward.argtypes = [p, p, p, p, p, p, i, i, i, i, f, p]
         L.dvmvs_lstm_gates_backward.argtypes = [p, p, p, p, p, p, i, i, i, i, p]

@@ -16,7 +16,12 @@ csrc/mesh.cu and tools/gen_mc_tables.py.  `get_mesh_tensors` leaves the mesh on 
 
 Rendering (`render` / `render_tensors`), which the reference lacks: depth, normal and colour maps of the fused model at any
 camera poses, ray-cast on the device by dvmvs_tsdf_raycast (csrc/raycast.cu, contract stated there), e.g. to score the fused
-depth against ground truth with dvmvs.errors.compute_errors or as model-to-frame depth for tracking."""
+depth against ground truth with dvmvs.errors.compute_errors or as model-to-frame depth for tracking.
+
+`SparseTSDFVolume`, which the reference lacks, fuses frames without bounds known up front (an online camera): voxel blocks are
+allocated on the device as frames see them (csrc/tsdf_sparse.cu) and hold what a TSDFVolume with the same origin holds after
+the same frames; `to_dense` exports any lattice-aligned box of it as a TSDFVolume for meshing and rendering."""
+import contextlib
 import ctypes
 
 import numpy as np
@@ -26,7 +31,60 @@ from . import _native as N
 from ._ops import _stream
 
 
-class TSDFVolume(object):
+class _FrameInputs(object):
+    """Frame inputs of integrate on the volume's device: numpy arrays through pinned staging, CUDA tensors in place."""
+
+    def _upload(self, a, name):
+        """Host array -> device through a two-deep ring of pinned staging buffers owned by the volume (allocating pinned
+        memory per frame would cost more than the kernel); a slot is reused only after its previous copy has completed."""
+        key = (name, tuple(a.shape), a.dtype)
+        ring = self._staging.get(key)
+        if ring is None:
+            ring = self._staging[key] = {"next": 0, "slots": [
+                (torch.empty(a.shape, dtype=a.dtype).pin_memory(), torch.empty(a.shape, dtype=a.dtype, device=self.device), torch.cuda.Event())
+                for _ in range(2)]}
+        host, dev, done = ring["slots"][ring["next"]]
+        ring["next"] ^= 1
+        done.synchronize()
+        host.copy_(a)
+        dev.copy_(host, non_blocking=True)
+        done.record()
+        return dev
+
+    def _to_device(self, a, allowed, name):
+        if isinstance(a, np.ndarray):
+            a = torch.from_numpy(np.ascontiguousarray(a))
+        if not isinstance(a, torch.Tensor):
+            raise TypeError("%s.integrate: %s must be a numpy array or a tensor" % (type(self).__name__, name))
+        if a.dtype not in allowed:
+            a = a.to(allowed[-1])
+        if not a.is_cuda:
+            return self._upload(a, name)
+        if a.device != self.device:
+            raise RuntimeError("%s.integrate: %s lives on %s, the volume on %s" % (type(self).__name__, name, a.device, self.device))
+        return a.contiguous()
+
+    def _frame(self, color_im, depth_im):
+        """(colour, depth) on the device, checked for shape"""
+        depth = self._to_device(depth_im, (torch.float64, torch.float32), "depth_im")
+        color = self._to_device(color_im, (torch.uint8, torch.float32), "color_im")
+        if depth.dim() != 2 or tuple(color.shape) != (depth.shape[0], depth.shape[1], 3):
+            raise RuntimeError("%s.integrate: expected depth (H,W) and colour (H,W,3), got %s and %s" % (
+                type(self).__name__, tuple(depth.shape), tuple(color.shape)))
+        return color, depth
+
+    @staticmethod
+    def _camera(cam_intr, cam_pose):
+        """(float32 fx, fy, cx, cy, float64 inv(cam_pose)) as ctypes arrays, computed on the host as in the reference"""
+        intr = np.asarray(cam_intr.cpu() if isinstance(cam_intr, torch.Tensor) else cam_intr).astype(np.float32)      # :197
+        pose = np.asarray(cam_pose.cpu() if isinstance(cam_pose, torch.Tensor) else cam_pose)
+        inv = np.ascontiguousarray(np.linalg.inv(pose), dtype=np.float64)              # :285, host logic as in the reference
+        intr4 = (ctypes.c_float * 4)(float(intr[0, 0]), float(intr[1, 1]), float(intr[0, 2]), float(intr[1, 2]))
+        inv16 = (ctypes.c_double * 16)(*[float(v) for v in inv.reshape(-1)])
+        return intr4, inv16
+
+
+class TSDFVolume(_FrameInputs):
     """Volumetric TSDF fusion of RGB-D frames (run-tsdf-reconstruction.py:30-358)."""
 
     def __init__(self, vol_bnds, voxel_size, use_gpu=True, device=None):
@@ -57,49 +115,12 @@ class TSDFVolume(object):
         self.gpu_mode = True
 
     # ---- the hot path -------------------------------------------------------------------------------------------------
-    def _upload(self, a, name):
-        """Host array -> device through a two-deep ring of pinned staging buffers owned by the volume (allocating pinned
-        memory per frame would cost more than the kernel); a slot is reused only after its previous copy has completed."""
-        key = (name, tuple(a.shape), a.dtype)
-        ring = self._staging.get(key)
-        if ring is None:
-            ring = self._staging[key] = {"next": 0, "slots": [
-                (torch.empty(a.shape, dtype=a.dtype).pin_memory(), torch.empty(a.shape, dtype=a.dtype, device=self.device), torch.cuda.Event())
-                for _ in range(2)]}
-        host, dev, done = ring["slots"][ring["next"]]
-        ring["next"] ^= 1
-        done.synchronize()
-        host.copy_(a)
-        dev.copy_(host, non_blocking=True)
-        done.record()
-        return dev
-
-    def _to_device(self, a, allowed, name):
-        if isinstance(a, np.ndarray):
-            a = torch.from_numpy(np.ascontiguousarray(a))
-        if not isinstance(a, torch.Tensor):
-            raise TypeError("TSDFVolume.integrate: %s must be a numpy array or a tensor" % name)
-        if a.dtype not in allowed:
-            a = a.to(allowed[-1])
-        if not a.is_cuda:
-            return self._upload(a, name)
-        if a.device != self.device:
-            raise RuntimeError("TSDFVolume.integrate: %s lives on %s, the volume on %s" % (name, a.device, self.device))
-        return a.contiguous()
-
     def integrate(self, color_im, depth_im, cam_intr, cam_pose, obs_weight=1.):
         """Integrate an RGB-D frame (:220-323).  color_im (H,W,3) RGB uint8 / float; depth_im (H,W) float32 / float64, 0 =
         invalid; cam_intr (3,3); cam_pose (4,4) camera-to-world; obs_weight: weight of this observation."""
-        intr = np.asarray(cam_intr.cpu() if isinstance(cam_intr, torch.Tensor) else cam_intr).astype(np.float32)      # :197
-        pose = np.asarray(cam_pose.cpu() if isinstance(cam_pose, torch.Tensor) else cam_pose)
-        inv = np.ascontiguousarray(np.linalg.inv(pose), dtype=np.float64)              # :285, host logic as in the reference
-        intr4 = (ctypes.c_float * 4)(float(intr[0, 0]), float(intr[1, 1]), float(intr[0, 2]), float(intr[1, 2]))
-        inv16 = (ctypes.c_double * 16)(*[float(v) for v in inv.reshape(-1)])
+        intr4, inv16 = self._camera(cam_intr, cam_pose)
         with torch.cuda.device(self.device):
-            depth = self._to_device(depth_im, (torch.float64, torch.float32), "depth_im")
-            color = self._to_device(color_im, (torch.uint8, torch.float32), "color_im")
-            if depth.dim() != 2 or tuple(color.shape) != (depth.shape[0], depth.shape[1], 3):
-                raise RuntimeError("TSDFVolume.integrate: expected depth (H,W) and colour (H,W,3), got %s and %s" % (tuple(depth.shape), tuple(color.shape)))
+            color, depth = self._frame(color_im, depth_im)
             N.check(N.lib().dvmvs_tsdf_integrate(
                 self._tsdf_vol.data_ptr(), self._weight_vol.data_ptr(), self._color_vol.data_ptr(),
                 int(self._vol_dim[0]), int(self._vol_dim[1]), int(self._vol_dim[2]), self._origin_c, self._voxel_size,
@@ -208,6 +229,157 @@ class TSDFVolume(object):
     def render(self, cam_intr, cam_poses, height, width):
         """render_tensors copied to the host: (depth, normals, colors) numpy arrays."""
         return tuple(t.cpu().numpy() for t in self.render_tensors(cam_intr, cam_poses, height, width))
+
+
+class SparseTSDFVolume(_FrameInputs):
+    """TSDF fusion without bounds: a volume of 8 x 8 x 8-voxel blocks on the device (csrc/tsdf_sparse.cu, C ABI
+    include/dvmvs_tsdf_sparse.h).  A frame allocates, through a hash table on the device, every block holding a voxel it can
+    update (free space in front of the surface included) and integrates only the blocks it sees, so memory grows with the
+    observed space and the work per frame with what the camera sees.  Voxel (i, j, k) of the signed global lattice sits at
+    f32(f64(origin) + voxel_size * f64((i, j, k))) and is updated by the arithmetic of TSDFVolume.integrate: after any frames
+    the volume holds, voxel for voxel, the tsdf, weight and colour a TSDFVolume whose origin is `origin` holds after the same
+    frames.  `to_dense` exports it into a TSDFVolume (for get_mesh / render).
+
+    Allocation runs on the device; integrate reads nothing back.  A pool of capacity_blocks blocks is allocated up front
+    (device_bytes tells its size).  When a frame needs more blocks than the pool holds, the blocks without room are not
+    integrated and the next allocated_blocks / to_dense raises RuntimeError naming the capacity the frames need; the blocks
+    that have room keep being integrated correctly."""
+    BLOCK = 8
+
+    @staticmethod
+    def table_size(capacity_blocks):
+        """hash-table entries for a pool of capacity_blocks blocks: the smallest power of two >= 2 * capacity_blocks"""
+        return 1 << max(1, (2 * int(capacity_blocks) - 1).bit_length())
+
+    @staticmethod
+    def device_bytes(capacity_blocks):
+        """device memory of a volume with capacity_blocks blocks: 512 voxels x 12 B, block coordinates and the visible list
+        per block; 8 B key and 4 B slot per hash-table entry; the counters"""
+        c = int(capacity_blocks)
+        return c * (SparseTSDFVolume.BLOCK ** 3 * 12 + 12 + 4) + SparseTSDFVolume.table_size(c) * 12 + 16
+
+    def __init__(self, voxel_size, origin=(0.0, 0.0, 0.0), capacity_blocks=32768, device=None):
+        voxel_size = float(voxel_size)
+        if not (np.isfinite(voxel_size) and voxel_size > 0):
+            raise ValueError("SparseTSDFVolume: voxel_size must be finite and > 0, got %r" % voxel_size)
+        origin = np.asarray(origin, dtype=np.float64)
+        if origin.shape != (3,) or not np.all(np.isfinite(origin)):
+            raise ValueError("SparseTSDFVolume: origin must be 3 finite numbers, got %r" % (origin,))
+        if isinstance(capacity_blocks, bool) or int(capacity_blocks) != capacity_blocks or capacity_blocks < 1:
+            raise ValueError("SparseTSDFVolume: capacity_blocks must be a positive integer, got %r" % (capacity_blocks,))
+        capacity = int(capacity_blocks)
+        if self.table_size(capacity) > 1 << 30:
+            raise ValueError("SparseTSDFVolume: capacity_blocks %d exceeds 2^29" % capacity)
+        if not N.DRYRUN and not torch.cuda.is_available():
+            raise RuntimeError("SparseTSDFVolume: needs a CUDA device (no CPU fallback)")
+        self._voxel_size = voxel_size
+        self._trunc_margin = 5 * voxel_size                                             # as TSDFVolume (:46)
+        self._origin = origin.astype(np.float32)
+        self._origin_c = (ctypes.c_float * 3)(*[float(v) for v in self._origin])
+        self.capacity = capacity
+        self.device = torch.device(device if device is not None else "cuda")
+        if self.device.type == "cuda" and self.device.index is None and torch.cuda.is_available():
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        dev, b = self.device, self.BLOCK
+        table = self.table_size(capacity)
+        self._keys = torch.full((table,), -1, dtype=torch.int64, device=dev)             # all bits set: empty
+        self._slots = torch.full((table,), -1, dtype=torch.int32, device=dev)
+        self._coords = torch.zeros((capacity, 3), dtype=torch.int32, device=dev)
+        self._tsdf = torch.ones((capacity, b, b, b), dtype=torch.float32, device=dev)   # TSDFVolume's initial state (:57-61)
+        self._weight = torch.zeros((capacity, b, b, b), dtype=torch.float32, device=dev)
+        self._color = torch.zeros((capacity, b, b, b), dtype=torch.float32, device=dev)
+        self._counters = torch.zeros(4, dtype=torch.int32, device=dev)                 # keys, flags, visible, unused
+        self._visible = torch.zeros(capacity, dtype=torch.int32, device=dev)
+        self._updated = torch.zeros(1, dtype=torch.int64, device=dev)
+        self._scratch = {}
+        self._staging = {}
+
+    def _device_scope(self):
+        return torch.cuda.device(self.device) if self.device.type == "cuda" else contextlib.nullcontext()
+
+    # ---- the hot path -------------------------------------------------------------------------------------------------
+    def integrate(self, color_im, depth_im, cam_intr, cam_pose, obs_weight=1.):
+        """Integrate an RGB-D frame: TSDFVolume.integrate's arguments, accepted types and arithmetic (:220-323), with the
+        blocks the frame can update allocated first.  Focal lengths must be finite and > 0."""
+        intr4, inv16 = self._camera(cam_intr, cam_pose)
+        if not (np.all(np.isfinite(list(intr4))) and intr4[0] > 0 and intr4[1] > 0):
+            raise ValueError("SparseTSDFVolume.integrate: focal lengths must be finite and > 0 and the principal point finite, "
+                             "got fx %r fy %r cx %r cy %r" % tuple(intr4))
+        with self._device_scope():
+            color, depth = self._frame(color_im, depth_im)
+            h, w = int(depth.shape[0]), int(depth.shape[1])
+            scratch = self._scratch.get((h, w))
+            if scratch is None:
+                nbytes = ctypes.c_longlong(0)
+                N.check(N.lib().dvmvs_tsdf_sparse_scratch_bytes(h, w, ctypes.byref(nbytes)), "tsdf_sparse_scratch_bytes")
+                scratch = self._scratch[(h, w)] = torch.empty(max(int(nbytes.value), 8), dtype=torch.uint8, device=self.device)
+            depth_f64 = 1 if depth.dtype == torch.float64 else 0
+            stream = _stream()
+            N.check(N.lib().dvmvs_tsdf_sparse_allocate(
+                self._keys.data_ptr(), self._slots.data_ptr(), int(self._keys.numel()), self._coords.data_ptr(), self.capacity,
+                self._counters.data_ptr(), self._visible.data_ptr(), scratch.data_ptr(), scratch.numel(), self._origin_c,
+                self._voxel_size, self._trunc_margin, depth.data_ptr(), depth_f64, h, w, intr4, inv16, stream), "tsdf_sparse_allocate")
+            N.check(N.lib().dvmvs_tsdf_sparse_integrate(
+                self._tsdf.data_ptr(), self._weight.data_ptr(), self._color.data_ptr(), self._coords.data_ptr(), self.capacity,
+                self._counters.data_ptr(), self._visible.data_ptr(), self._origin_c, self._voxel_size, self._trunc_margin,
+                color.data_ptr(), 1 if color.dtype == torch.uint8 else 0, depth.data_ptr(), depth_f64, h, w, intr4, inv16,
+                float(obs_weight), self._updated.data_ptr(), stream), "tsdf_sparse_integrate")
+
+    # ---- read-back ----------------------------------------------------------------------------------------------------
+    def allocated_blocks(self):
+        """Number of blocks allocated so far (synchronises).  RuntimeError when a frame found no room for a block."""
+        n, flags = (int(v) for v in self._counters[:2].cpu())
+        if flags & N.SPARSE_TABLE_FULL:
+            raise RuntimeError("SparseTSDFVolume: the hash table of %d entries is full; the frames so far need more than %d "
+                               "blocks: construct the volume with a larger capacity_blocks" % (self._keys.numel(), n))
+        if flags & N.SPARSE_POOL_FULL:
+            raise RuntimeError("SparseTSDFVolume: the frames so far need %d blocks, the pool holds %d: construct the volume with "
+                               "capacity_blocks >= %d" % (n, self.capacity, n))
+        if flags & N.SPARSE_FRUSTUM:
+            raise RuntimeError("SparseTSDFVolume: a frame was not integrated: its view frustum, to its largest depth, spans more "
+                               "than 2^31 blocks or leaves the block coordinate range +-2^20")
+        return n
+
+    def updated_voxels(self):
+        """Total number of voxel updates so far (synchronises)."""
+        return int(self._updated.item())
+
+    def to_dense(self, vol_bnds=None):
+        """The volume as a TSDFVolume over vol_bnds ((3,2) metres, as TSDFVolume's; the lower bounds on the voxel lattice
+        origin + k * voxel_size, else ValueError), by default the bounding box of the allocated blocks.  Voxels of no allocated
+        block hold TSDFVolume's initial 1 / 0 / 0.  RuntimeError as allocated_blocks."""
+        n = self.allocated_blocks()
+        vs, origin = self._voxel_size, self._origin.astype(np.float64)
+        if vol_bnds is None:
+            if n == 0:
+                raise ValueError("SparseTSDFVolume.to_dense: no block is allocated; give vol_bnds")
+            bounds = torch.empty(6, dtype=torch.int32, device=self.device)
+            with self._device_scope():
+                N.check(N.lib().dvmvs_tsdf_sparse_block_bounds(self._coords.data_ptr(), self.capacity, self._counters.data_ptr(),
+                                                                bounds.data_ptr(), _stream()), "tsdf_sparse_block_bounds")
+            b = bounds.cpu().numpy().astype(np.int64)
+            k = b[:3] * self.BLOCK
+            dims = (b[3:] - b[:3] + 1) * self.BLOCK
+            lo = origin + k * vs
+            vol_bnds = np.stack([lo, lo + (dims - 0.5) * vs], axis=1)                  # TSDFVolume's ceil gives dims exactly
+        vol_bnds = np.array(vol_bnds, dtype=np.float64)
+        if vol_bnds.shape != (3, 2) or not np.all(np.isfinite(vol_bnds)):
+            raise ValueError("SparseTSDFVolume.to_dense: vol_bnds must be (3,2) finite bounds, got %r" % (vol_bnds,))
+        k = np.rint((vol_bnds[:, 0] - origin) / vs)
+        off = np.abs(vol_bnds[:, 0] - (origin + k * vs))
+        if np.any(off > 1e-3 * vs + 2.0 ** -23 * np.abs(vol_bnds[:, 0])) or np.any(np.abs(k) >= 2 ** 31):
+            raise ValueError("SparseTSDFVolume.to_dense: the lower bounds %s are not on the voxel lattice origin %s + k * %r"
+                             % (vol_bnds[:, 0].tolist(), origin.tolist(), vs))
+        dense = TSDFVolume(vol_bnds, vs, device=self.device)
+        dims = [int(d) for d in dense._vol_dim]
+        if min(dims) > 0:
+            tsdf, weight, color = dense.get_volume_tensors()
+            with self._device_scope():
+                N.check(N.lib().dvmvs_tsdf_sparse_export(
+                    self._tsdf.data_ptr(), self._weight.data_ptr(), self._color.data_ptr(), self._coords.data_ptr(), self.capacity,
+                    self._counters.data_ptr(), (ctypes.c_int * 3)(*[int(v) for v in k]), dims[0], dims[1], dims[2],
+                    tsdf.data_ptr(), weight.data_ptr(), color.data_ptr(), _stream()), "tsdf_sparse_export")
+        return dense
 
 
 class TSDFFusion(object):
