@@ -24,9 +24,9 @@
 #include <limits.h>
 #include <math.h>
 
-#include "color_fold.cuh"
 #include "common.cuh"
 #include "mc_tables.cuh"
+#include "mc_vertex.cuh"
 
 namespace dvmvs {
 
@@ -43,8 +43,6 @@ struct VoxelClass {
   unsigned edges;                  // bit a: the voxel's +a grid edge crosses
   float f0, fe[3];                 // tsdf at the voxel and at its +x / +y / +z neighbours
 };
-
-__device__ __forceinline__ bool mc_inside(float v) { return v < 0.f; }   // NaN is never inside
 
 __device__ __forceinline__ int mc_corner_offset(const MeshGrid& g, int c) {
   return (c & 1) * g.sx + ((c >> 1) & 1) * g.dz + ((c >> 2) & 1);
@@ -156,40 +154,23 @@ struct MeshEmitParams {
   int* faces;                      // [F][3], edge keys until mesh_resolve_kernel
 };
 
-// np.gradient of the volume at voxel (x, y, z), float32: (f[i+1] - f[i-1]) / 2 inside, f[1] - f[0] and f[n-1] - f[n-2] at
-// the border (every dimension is >= 2 here)
 __device__ __forceinline__ void mc_gradient(const MeshEmitParams& p, int x, int y, int z, float* gr) {
   const int q[3] = {x, y, z}, dim[3] = {p.g.dx, p.g.dy, p.g.dz}, step[3] = {p.g.sx, p.g.dz, 1};
   const int lin = x * p.g.sx + y * p.g.dz + z;
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    if (q[a] == 0) gr[a] = __fsub_rn(p.tsdf[lin + step[a]], p.tsdf[lin]);
-    else if (q[a] == dim[a] - 1) gr[a] = __fsub_rn(p.tsdf[lin], p.tsdf[lin - step[a]]);
-    else gr[a] = __fdiv_rn(__fsub_rn(p.tsdf[lin + step[a]], p.tsdf[lin - step[a]]), 2.f);
-  }
+  mc_np_gradient(q, dim, [&](int a, int s) { return p.tsdf[lin + s * step[a]]; }, gr);
 }
 
 __device__ __forceinline__ void mc_emit_vertex(const MeshEmitParams& p, const VoxelClass& v, int axis, int slot) {
-  const float a = v.f0, b = v.fe[axis];
-  const float t = __fdiv_rn(-a, __fsub_rn(b, a));
-  float vi[3] = {(float)v.x, (float)v.y, (float)v.z};
-  vi[axis] = __fadd_rn(vi[axis], t);
-  float ga[3], gb[3], nrm[3];
-  mc_gradient(p, v.x, v.y, v.z, ga);
-  mc_gradient(p, v.x + (axis == 0), v.y + (axis == 1), v.z + (axis == 2), gb);
-#pragma unroll
-  for (int c = 0; c < 3; ++c) nrm[c] = __fadd_rn(ga[c], __fmul_rn(t, __fsub_rn(gb[c], ga[c])));
-  const float len = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(nrm[0], nrm[0]), __fmul_rn(nrm[1], nrm[1])), __fmul_rn(nrm[2], nrm[2])));
-  const int ix = (int)rintf(vi[0]), iy = (int)rintf(vi[1]), iz = (int)rintf(vi[2]);
-  float cb, cg, cr;
-  unfold(p.color[(size_t)ix * p.g.sx + (size_t)iy * p.g.dz + iz], cb, cg, cr);
-  const float rgb[3] = {cr, cg, cb};
+  const int q[3] = {v.x, v.y, v.z};
+  const McVertex m = mc_vertex(v.f0, v.fe[axis], q, axis, [&](int x, int y, int z, float* gr) { mc_gradient(p, x, y, z, gr); },
+                               [&](int ix, int iy, int iz) { return p.color[(size_t)ix * p.g.sx + (size_t)iy * p.g.dz + iz]; }, p.origin,
+                               p.voxel);
   const size_t o = (size_t)slot * 3;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    p.verts[o + c] = __fadd_rn(__fmul_rn(vi[c], p.voxel), p.origin[c]);
-    p.norms[o + c] = len > 0.f ? __fdiv_rn(nrm[c], len) : 0.f;
-    p.colors[o + c] = (unsigned char)__float2int_rz(floorf(rgb[c]));     // numpy's float -> uint8 cast (truncation)
+    p.verts[o + c] = m.vert[c];
+    p.norms[o + c] = m.norm[c];
+    p.colors[o + c] = m.rgb[c];
   }
   p.keys[slot] = 3 * v.lin + axis;
 }

@@ -32,14 +32,13 @@
 #include <limits.h>
 #include <math.h>
 
-#include "color_fold.cuh"
 #include "common.cuh"
+#include "raycast_march.cuh"
 
 namespace dvmvs {
 
 constexpr int kRayTileW = 16, kRayTileH = 8;       // pixels per CTA; 4 warps of 8 x 4
 constexpr int kRayMaxViewsPerLaunch = 65535;       // gridDim.y
-constexpr float kRayMaxSamples = 1073741824.f;     // 2^30: lattices longer than this (only degenerate poses) give no hits
 
 struct RaycastParams {
   const float* tsdf;
@@ -54,53 +53,6 @@ struct RaycastParams {
   float voxel;
 };
 
-__device__ __forceinline__ float rc_lerp(float a, float b, float f) { return __fadd_rn(a, __fmul_rn(f, __fsub_rn(b, a))); }
-
-struct RayCell {
-  float c[8];                      // corner (i, j, k) at c[i + 2 j + 4 k]
-  float f[3];
-};
-
-// the cell and fractions of the point o + z d (clamped into the box) and its 8 corners
-__device__ __forceinline__ void rc_cell(const RaycastParams& p, const float* o, const float* d, float z, RayCell& cell) {
-  int ci[3];
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    const float g = fminf(fmaxf(__fadd_rn(o[a], __fmul_rn(z, d[a])), 0.f), (float)(p.dim[a] - 1));
-    ci[a] = min((int)floorf(g), p.dim[a] - 2);
-    cell.f[a] = __fsub_rn(g, (float)ci[a]);
-  }
-  const size_t sx = (size_t)p.dim[1] * p.dim[2], sy = (size_t)p.dim[2];
-  const float* b = p.tsdf + (size_t)ci[0] * sx + (size_t)ci[1] * sy + ci[2];
-#pragma unroll
-  for (int k = 0; k < 2; ++k)
-#pragma unroll
-    for (int j = 0; j < 2; ++j)
-#pragma unroll
-      for (int i = 0; i < 2; ++i) cell.c[i + 2 * j + 4 * k] = __ldg(b + i * sx + j * sy + k);
-}
-
-__device__ __forceinline__ float rc_trilinear(const RayCell& s) {
-  const float x00 = rc_lerp(s.c[0], s.c[1], s.f[0]), x10 = rc_lerp(s.c[2], s.c[3], s.f[0]);
-  const float x01 = rc_lerp(s.c[4], s.c[5], s.f[0]), x11 = rc_lerp(s.c[6], s.c[7], s.f[0]);
-  return rc_lerp(rc_lerp(x00, x10, s.f[1]), rc_lerp(x01, x11, s.f[1]), s.f[2]);
-}
-
-__device__ __forceinline__ bool rc_all_ones(const RayCell& s) {
-  bool ones = true;
-#pragma unroll
-  for (int c = 0; c < 8; ++c) ones = ones && s.c[c] == 1.f;
-  return ones;
-}
-
-// F at lattice sample k; *ones = the sample's cell is fully truncated
-__device__ __forceinline__ float rc_sample(const RaycastParams& p, const float* o, const float* d, float z_near, float dz, int k, bool* ones) {
-  RayCell s;
-  rc_cell(p, o, d, __fadd_rn(z_near, __fmul_rn((float)k, dz)), s);
-  *ones = rc_all_ones(s);
-  return rc_trilinear(s);
-}
-
 __global__ void __launch_bounds__(kRayTileW * kRayTileH) raycast_kernel(RaycastParams p) {
   pdl_launch_dependents();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -113,92 +65,35 @@ __global__ void __launch_bounds__(kRayTileW * kRayTileH) raycast_kernel(RaycastP
   float vw[16];
 #pragma unroll
   for (int i = 0; i < 16; ++i) vw[i] = __ldg(view + i);
-  const float dcx = __fdiv_rn(__fsub_rn((float)u, vw[2]), vw[0]);
-  const float dcy = __fdiv_rn(__fsub_rn((float)v, vw[3]), vw[1]);
-  float o[3], d[3];
+  const Ray r = rc_ray(vw, u, v, p.dim, p.origin, p.voxel);
+  const size_t sx = (size_t)p.dim[1] * p.dim[2], sy = (size_t)p.dim[2];
+  const auto corners = [&](const int* ci, float* c) {
+    const float* b = p.tsdf + (size_t)ci[0] * sx + (size_t)ci[1] * sy + ci[2];
 #pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    const float w = __fadd_rn(__fadd_rn(__fmul_rn(vw[4 + 3 * a], dcx), __fmul_rn(vw[5 + 3 * a], dcy)), vw[6 + 3 * a]);
-    d[a] = __fdiv_rn(w, p.voxel);
-    o[a] = __fdiv_rn(__fsub_rn(vw[13 + a], p.origin[a]), p.voxel);
-  }
-  const float len = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2])));
-  const float dz = __fdiv_rn(0.5f, len);
-  bool inside_box = p.dim[0] >= 2 && p.dim[1] >= 2 && p.dim[2] >= 2;
-  float z_near = 0.f, z_far = INFINITY;
+    for (int k = 0; k < 2; ++k)
 #pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    const float hi = (float)(p.dim[a] - 1);
-    if (d[a] == 0.f) {
-      inside_box = inside_box && o[a] >= 0.f && o[a] <= hi;
-    } else {
-      const float t0 = __fdiv_rn(-o[a], d[a]), t1 = __fdiv_rn(__fsub_rn(hi, o[a]), d[a]);
-      z_near = fmaxf(z_near, fminf(t0, t1));
-      z_far = fminf(z_far, fmaxf(t0, t1));
-    }
-  }
+      for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) c[i + 2 * j + 4 * k] = __ldg(b + i * sx + j * sy + k);
+  };
   float z_hit = 0.f;
-  bool hit = false;
-  const float n_f = floorf(__fdiv_rn(__fsub_rn(z_far, z_near), dz));
-  if (inside_box && z_near <= z_far && n_f < kRayMaxSamples) {     // false for NaN (a degenerate pose)
-    const int n = (int)n_f;
-    bool ones;
-    float f_prev = rc_sample(p, o, d, z_near, dz, 0, &ones);
-    int k = 0;
-    while (k < n) {
-      if (ones && k + p.n_skip <= n) {
-        bool ones_j;
-        const float f_j = rc_sample(p, o, d, z_near, dz, k + p.n_skip, &ones_j);
-        if (!(f_j < 0.f)) {
-          k += p.n_skip;
-          f_prev = f_j;
-          ones = ones_j;
-          continue;
-        }
-      }
-      const float f_cur = rc_sample(p, o, d, z_near, dz, k + 1, &ones);
-      if (f_prev >= 0.f && f_cur < 0.f) {
-        const float z_prev = __fadd_rn(z_near, __fmul_rn((float)k, dz));
-        z_hit = __fadd_rn(z_prev, __fdiv_rn(__fmul_rn(dz, f_prev), __fsub_rn(f_prev, f_cur)));
-        hit = true;
-        break;
-      }
-      f_prev = f_cur;
-      ++k;
-    }
-  }
+  const bool hit = rc_march(p.dim, r, p.n_skip, corners, &z_hit);
   const size_t pix = ((size_t)blockIdx.y * p.im_h + v) * p.im_w + u;
-  float nrm[3] = {0.f, 0.f, 0.f}, rgb[3] = {0.f, 0.f, 0.f};
+  float nrm[3] = {0.f, 0.f, 0.f};
+  unsigned char rgb[3] = {0, 0, 0};
   if (hit) {
     RayCell s;
-    rc_cell(p, o, d, z_hit, s);
-    const float* c = s.c;
-    const float* f = s.f;
-    // x differences over (y, z), y differences over (x, z), z differences over (x, y)
-    const float gx = rc_lerp(rc_lerp(__fsub_rn(c[1], c[0]), __fsub_rn(c[3], c[2]), f[1]), rc_lerp(__fsub_rn(c[5], c[4]), __fsub_rn(c[7], c[6]), f[1]), f[2]);
-    const float gy = rc_lerp(rc_lerp(__fsub_rn(c[2], c[0]), __fsub_rn(c[3], c[1]), f[0]), rc_lerp(__fsub_rn(c[6], c[4]), __fsub_rn(c[7], c[5]), f[0]), f[2]);
-    const float gz = rc_lerp(rc_lerp(__fsub_rn(c[4], c[0]), __fsub_rn(c[5], c[1]), f[0]), rc_lerp(__fsub_rn(c[6], c[2]), __fsub_rn(c[7], c[3]), f[0]), f[1]);
-    const float glen = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(gx, gx), __fmul_rn(gy, gy)), __fmul_rn(gz, gz)));
-    if (glen > 0.f) {
-      nrm[0] = __fdiv_rn(gx, glen);
-      nrm[1] = __fdiv_rn(gy, glen);
-      nrm[2] = __fdiv_rn(gz, glen);
-    }
+    rc_cell(p.dim, r.o, r.d, z_hit, corners, s);
+    rc_normal(s, nrm);
     int vi[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a)
-      vi[a] = (int)rintf(fminf(fmaxf(__fadd_rn(o[a], __fmul_rn(z_hit, d[a])), 0.f), (float)(p.dim[a] - 1)));
-    float cb, cg, cr;
-    unfold(p.color[((size_t)vi[0] * p.dim[1] + vi[1]) * p.dim[2] + vi[2]], cb, cg, cr);
-    rgb[0] = cr;
-    rgb[1] = cg;
-    rgb[2] = cb;
+    rc_color_voxel(p.dim, r, z_hit, vi);
+    rc_rgb(p.color[((size_t)vi[0] * p.dim[1] + vi[1]) * p.dim[2] + vi[2]], rgb);
   }
   p.depth[pix] = z_hit;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
     p.normals[pix * 3 + c] = nrm[c];
-    p.colors[pix * 3 + c] = (unsigned char)__float2int_rz(floorf(rgb[c]));     // numpy's float -> uint8 cast (truncation)
+    p.colors[pix * 3 + c] = rgb[c];
   }
 }
 
@@ -223,9 +118,7 @@ extern "C" int dvmvs_tsdf_raycast(const float* tsdf_vol, const float* color_vol,
   p.dim[2] = dim_z;
   p.im_h = im_h;
   p.im_w = im_w;
-  // trunc - (sqrt(3) / 2) voxel is the least distance to the surface of any point in a cell whose corners are all truncated
-  const double n_skip = floor((trunc_margin / voxel_size - 0.8660254037844386) / 0.5);
-  p.n_skip = (int)fmin(fmax(n_skip, 1.0), (double)(1 << 24));
+  p.n_skip = rc_n_skip(trunc_margin, voxel_size);
   for (int a = 0; a < 3; ++a) p.origin[a] = vol_origin3[a];
   p.voxel = (float)voxel_size;
   const int tiles = ((im_w + kRayTileW - 1) / kRayTileW) * ((im_h + kRayTileH - 1) / kRayTileH);

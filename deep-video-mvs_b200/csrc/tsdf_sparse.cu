@@ -24,16 +24,12 @@
 #include <math.h>
 
 #include "../../include/dvmvs_tsdf_sparse.h"
+#include "tsdf_block_hash.cuh"
 #include "tsdf_voxel.cuh"
 
 namespace dvmvs {
 
-constexpr int kBlock = 8;                            // voxels per block edge
-constexpr int kBlockVoxels = kBlock * kBlock * kBlock;
 constexpr int kTile = 16;                            // pixels per tile edge of the max-depth image
-constexpr int kKeyBits = 21;                         // per axis: block coordinates in [-2^20, 2^20)
-constexpr int kKeyBias = 1 << (kKeyBits - 1);
-constexpr unsigned long long kEmpty = ~0ull;         // bit 63 is never set in a key
 constexpr long long kMaxCandidates = 1ll << 31;
 constexpr int kBoxBytes = 64;                        // scratch head: SparseBox
 
@@ -61,17 +57,11 @@ struct SparseTable {
   int mask, capacity;
 };
 
-__device__ __forceinline__ unsigned long long block_key(int bx, int by, int bz) {
-  const unsigned long long m = (1ull << kKeyBits) - 1;
-  return (((unsigned long long)(bx + kKeyBias) & m) << (2 * kKeyBits)) | (((unsigned long long)(by + kKeyBias) & m) << kKeyBits) |
-         ((unsigned long long)(bz + kKeyBias) & m);
-}
-
 // the pool slot of the block (inserted if new), or -1 (pool or table full: flagged).  Within one launch every key is looked up
 // by one thread only, so a key found in the table was inserted by an earlier launch and its slot is published.
 __device__ int sparse_insert(const SparseTable& t, int bx, int by, int bz) {
   const unsigned long long key = block_key(bx, by, bz);
-  unsigned h = (unsigned)((key * 0x9E3779B97F4A7C15ull) >> 32) & (unsigned)t.mask;
+  unsigned h = block_hash(key, t.mask);
   for (int probe = 0; probe <= t.mask; ++probe, h = (h + 1) & (unsigned)t.mask) {
     unsigned long long k = t.keys[h];                // a stale read can only be kEmpty: the CAS below then sees the truth
     if (k == kEmpty) k = atomicCAS(&t.keys[h], kEmpty, key);

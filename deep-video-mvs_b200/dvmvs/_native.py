@@ -32,6 +32,11 @@ SPARSE_SYMBOLS = [
     "dvmvs_tsdf_sparse_block_bounds",
 ]
 SPARSE_POOL_FULL, SPARSE_TABLE_FULL, SPARSE_FRUSTUM = 1, 2, 4
+# every symbol include/dvmvs_tsdf_sparse_view.h declares (mesh and ray casting of the voxel-block volume on its blocks;
+# tests/test_tsdf_sparse_view.py covers them)
+SPARSE_VIEW_SYMBOLS = [
+    "dvmvs_tsdf_sparse_mesh_scratch_bytes", "dvmvs_tsdf_sparse_mesh_count", "dvmvs_tsdf_sparse_mesh_extract", "dvmvs_tsdf_sparse_raycast",
+]
 
 
 class ConvDesc(ctypes.Structure):
@@ -151,6 +156,11 @@ def lib():
                                                   ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_double), d, p, p]
         L.dvmvs_tsdf_sparse_export.argtypes = [p, p, p, p, i, p, ctypes.POINTER(ctypes.c_int), i, i, i, p, p, p, p]
         L.dvmvs_tsdf_sparse_block_bounds.argtypes = [p, i, p, p, p]
+        llp, fp3 = ctypes.POINTER(ll), ctypes.POINTER(ctypes.c_float)
+        L.dvmvs_tsdf_sparse_mesh_scratch_bytes.argtypes = [i, llp]
+        L.dvmvs_tsdf_sparse_mesh_count.argtypes = [p, p, i, p, i, p, p, i, llp, i, i, i, p, ll, p]
+        L.dvmvs_tsdf_sparse_mesh_extract.argtypes = [p, p, i, p, i, p, p, p, i, llp, i, i, i, fp3, f, p, ll, i, i, p, p, p, p, p, p]
+        L.dvmvs_tsdf_sparse_raycast.argtypes = [p, p, i, p, i, p, p, p, llp, i, i, i, fp3, d, d, p, i, i, i, p, p, p, p]
         L.dvmvs_plane_sweep_backward.argtypes = [p, p, p, p, p, p, p, p, i, i, i, i, i, i, f, f, i, p]
         L.dvmvs_hidden_warp_backward.argtypes = [p, p, p, p, p, p, i, i, i, i, f, p]
         L.dvmvs_lstm_gates_backward.argtypes = [p, p, p, p, p, p, i, i, i, i, p]

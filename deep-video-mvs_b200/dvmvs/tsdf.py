@@ -20,7 +20,8 @@ depth against ground truth with dvmvs.errors.compute_errors or as model-to-frame
 
 `SparseTSDFVolume`, which the reference lacks, fuses frames without bounds known up front (an online camera): voxel blocks are
 allocated on the device as frames see them (csrc/tsdf_sparse.cu) and hold what a TSDFVolume with the same origin holds after
-the same frames; `to_dense` exports any lattice-aligned box of it as a TSDFVolume for meshing and rendering."""
+the same frames; `to_dense` exports any lattice-aligned box of it as a TSDFVolume, and its mesh and render methods return
+exactly what the export's would, computed on the blocks without the dense box (csrc/tsdf_sparse_view.cu)."""
 import contextlib
 import ctypes
 
@@ -82,6 +83,43 @@ class _FrameInputs(object):
         intr4 = (ctypes.c_float * 4)(float(intr[0, 0]), float(intr[1, 1]), float(intr[0, 2]), float(intr[1, 2]))
         inv16 = (ctypes.c_double * 16)(*[float(v) for v in inv.reshape(-1)])
         return intr4, inv16
+
+    def _views(self, cam_intr, cam_poses, height, width):
+        """render_tensors' arguments checked and packed: (views (V,16) float32 on the device -- fx fy cx cy, R row-major, t --,
+        V, whether a single (4,4) pose was given, height, width).  Call inside the volume's device scope."""
+        name = type(self).__name__
+        intr = np.asarray(cam_intr.detach().cpu() if isinstance(cam_intr, torch.Tensor) else cam_intr)
+        if intr.shape != (3, 3):
+            raise RuntimeError("%s.render: cam_intr must be (3,3), got %s" % (name, intr.shape))
+        intr4 = intr.astype(np.float32)[[0, 1, 0, 1], [0, 1, 2, 2]]                  # fx fy cx cy
+        if not (np.all(np.isfinite(intr4)) and intr4[0] > 0 and intr4[1] > 0):
+            raise RuntimeError("%s.render: focal lengths must be finite and > 0 and the principal point finite, got "
+                               "fx %r fy %r cx %r cy %r" % ((name,) + tuple(float(v) for v in intr4)))
+        height, width = int(height), int(width)
+        if height <= 0 or width <= 0:
+            raise RuntimeError("%s.render: bad image size %d x %d" % (name, height, width))
+        poses = cam_poses
+        if isinstance(poses, torch.Tensor) and poses.device.type == "cpu":
+            poses = poses.detach().numpy()
+        if not isinstance(poses, torch.Tensor):
+            poses = np.asarray(poses)
+        shape = tuple(poses.shape)
+        single = shape == (4, 4)
+        if not (single or (len(shape) == 3 and shape[0] > 0 and shape[1:] == (4, 4))):
+            raise RuntimeError("%s.render: cam_poses must be (4,4) or (V,4,4), got %s" % (name, shape))
+        n = 1 if single else shape[0]
+        if isinstance(poses, torch.Tensor):
+            if poses.device != self.device:
+                raise RuntimeError("%s.render: cam_poses lives on %s, the volume on %s" % (name, poses.device, self.device))
+            p = poses.detach().reshape(n, 4, 4)
+            intr_dev = self._upload(torch.from_numpy(intr4.copy()), "intr")             # pinned: no stream synchronisation
+            views = torch.cat([intr_dev.expand(n, 4), p[:, :3, :3].reshape(n, 9).to(torch.float32), p[:, :3, 3].to(torch.float32)],
+                              dim=1).contiguous()
+        else:
+            p = poses.reshape(n, 4, 4).astype(np.float32)
+            packed = np.concatenate([np.broadcast_to(intr4, (n, 4)), p[:, :3, :3].reshape(n, 9), p[:, :3, 3]], axis=1)
+            views = self._upload(torch.from_numpy(np.ascontiguousarray(packed, dtype=np.float32)), "views")
+        return views, n, single, height, width
 
 
 class TSDFVolume(_FrameInputs):
@@ -183,38 +221,8 @@ class TSDFVolume(_FrameInputs):
         camera depth of the first + -> - crossing of the tsdf (0 = no hit), normals (V,H,W,3) float32 world-frame unit normals
         toward increasing tsdf and colors (V,H,W,3) uint8 RGB (both 0 where there is no hit); a single (4,4) pose gives them
         without the V axis.  The raw tsdf is rendered: unobserved voxels are not masked (as in get_mesh)."""
-        intr = np.asarray(cam_intr.detach().cpu() if isinstance(cam_intr, torch.Tensor) else cam_intr)
-        if intr.shape != (3, 3):
-            raise RuntimeError("TSDFVolume.render: cam_intr must be (3,3), got %s" % (intr.shape,))
-        intr4 = intr.astype(np.float32)[[0, 1, 0, 1], [0, 1, 2, 2]]                  # fx fy cx cy
-        if not (np.all(np.isfinite(intr4)) and intr4[0] > 0 and intr4[1] > 0):
-            raise RuntimeError("TSDFVolume.render: focal lengths must be finite and > 0 and the principal point finite, got "
-                               "fx %r fy %r cx %r cy %r" % tuple(float(v) for v in intr4))
-        height, width = int(height), int(width)
-        if height <= 0 or width <= 0:
-            raise RuntimeError("TSDFVolume.render: bad image size %d x %d" % (height, width))
-        poses = cam_poses
-        if isinstance(poses, torch.Tensor) and poses.device.type == "cpu":
-            poses = poses.detach().numpy()
-        if not isinstance(poses, torch.Tensor):
-            poses = np.asarray(poses)
-        shape = tuple(poses.shape)
-        single = shape == (4, 4)
-        if not (single or (len(shape) == 3 and shape[0] > 0 and shape[1:] == (4, 4))):
-            raise RuntimeError("TSDFVolume.render: cam_poses must be (4,4) or (V,4,4), got %s" % (shape,))
-        n = 1 if single else shape[0]
         with torch.cuda.device(self.device):
-            if isinstance(poses, torch.Tensor):
-                if poses.device != self.device:
-                    raise RuntimeError("TSDFVolume.render: cam_poses lives on %s, the volume on %s" % (poses.device, self.device))
-                p = poses.detach().reshape(n, 4, 4)
-                intr_dev = self._upload(torch.from_numpy(intr4.copy()), "intr")             # pinned: no stream synchronisation
-                views = torch.cat([intr_dev.expand(n, 4), p[:, :3, :3].reshape(n, 9).to(torch.float32), p[:, :3, 3].to(torch.float32)],
-                                  dim=1).contiguous()
-            else:
-                p = poses.reshape(n, 4, 4).astype(np.float32)
-                packed = np.concatenate([np.broadcast_to(intr4, (n, 4)), p[:, :3, :3].reshape(n, 9), p[:, :3, 3]], axis=1)
-                views = self._upload(torch.from_numpy(np.ascontiguousarray(packed, dtype=np.float32)), "views")
+            views, n, single, height, width = self._views(cam_intr, cam_poses, height, width)
             depth = torch.empty((n, height, width), dtype=torch.float32, device=self.device)
             normals = torch.empty((n, height, width, 3), dtype=torch.float32, device=self.device)
             colors = torch.empty((n, height, width, 3), dtype=torch.uint8, device=self.device)
@@ -238,7 +246,8 @@ class SparseTSDFVolume(_FrameInputs):
     observed space and the work per frame with what the camera sees.  Voxel (i, j, k) of the signed global lattice sits at
     f32(f64(origin) + voxel_size * f64((i, j, k))) and is updated by the arithmetic of TSDFVolume.integrate: after any frames
     the volume holds, voxel for voxel, the tsdf, weight and colour a TSDFVolume whose origin is `origin` holds after the same
-    frames.  `to_dense` exports it into a TSDFVolume (for get_mesh / render).
+    frames.  `to_dense` exports it into a TSDFVolume; get_mesh / get_point_cloud / render compute what the export's would,
+    on the blocks.
 
     Allocation runs on the device; integrate reads nothing back.  A pool of capacity_blocks blocks is allocated up front
     (device_bytes tells its size).  When a frame needs more blocks than the pool holds, the blocks without room are not
@@ -344,15 +353,15 @@ class SparseTSDFVolume(_FrameInputs):
         """Total number of voxel updates so far (synchronises)."""
         return int(self._updated.item())
 
-    def to_dense(self, vol_bnds=None):
-        """The volume as a TSDFVolume over vol_bnds ((3,2) metres, as TSDFVolume's; the lower bounds on the voxel lattice
-        origin + k * voxel_size, else ValueError), by default the bounding box of the allocated blocks.  Voxels of no allocated
-        block hold TSDFVolume's initial 1 / 0 / 0.  RuntimeError as allocated_blocks."""
+    def _box(self, vol_bnds, what):
+        """(allocated blocks, lower global voxel index k (3,) int64, vol_bnds (3,2) float64) of a lattice-aligned box, by default
+        the bounding box of the allocated blocks.  RuntimeError as allocated_blocks; ValueError for a box off the lattice or no
+        default box."""
         n = self.allocated_blocks()
         vs, origin = self._voxel_size, self._origin.astype(np.float64)
         if vol_bnds is None:
             if n == 0:
-                raise ValueError("SparseTSDFVolume.to_dense: no block is allocated; give vol_bnds")
+                raise ValueError("SparseTSDFVolume.%s: no block is allocated; give vol_bnds" % what)
             bounds = torch.empty(6, dtype=torch.int32, device=self.device)
             with self._device_scope():
                 N.check(N.lib().dvmvs_tsdf_sparse_block_bounds(self._coords.data_ptr(), self.capacity, self._counters.data_ptr(),
@@ -364,13 +373,20 @@ class SparseTSDFVolume(_FrameInputs):
             vol_bnds = np.stack([lo, lo + (dims - 0.5) * vs], axis=1)                  # TSDFVolume's ceil gives dims exactly
         vol_bnds = np.array(vol_bnds, dtype=np.float64)
         if vol_bnds.shape != (3, 2) or not np.all(np.isfinite(vol_bnds)):
-            raise ValueError("SparseTSDFVolume.to_dense: vol_bnds must be (3,2) finite bounds, got %r" % (vol_bnds,))
+            raise ValueError("SparseTSDFVolume.%s: vol_bnds must be (3,2) finite bounds, got %r" % (what, vol_bnds))
         k = np.rint((vol_bnds[:, 0] - origin) / vs)
         off = np.abs(vol_bnds[:, 0] - (origin + k * vs))
         if np.any(off > 1e-3 * vs + 2.0 ** -23 * np.abs(vol_bnds[:, 0])) or np.any(np.abs(k) >= 2 ** 31):
-            raise ValueError("SparseTSDFVolume.to_dense: the lower bounds %s are not on the voxel lattice origin %s + k * %r"
-                             % (vol_bnds[:, 0].tolist(), origin.tolist(), vs))
-        dense = TSDFVolume(vol_bnds, vs, device=self.device)
+            raise ValueError("SparseTSDFVolume.%s: the lower bounds %s are not on the voxel lattice origin %s + k * %r"
+                             % (what, vol_bnds[:, 0].tolist(), origin.tolist(), vs))
+        return n, k.astype(np.int64), vol_bnds
+
+    def to_dense(self, vol_bnds=None):
+        """The volume as a TSDFVolume over vol_bnds ((3,2) metres, as TSDFVolume's; the lower bounds on the voxel lattice
+        origin + k * voxel_size, else ValueError), by default the bounding box of the allocated blocks.  Voxels of no allocated
+        block hold TSDFVolume's initial 1 / 0 / 0.  RuntimeError as allocated_blocks."""
+        _, k, vol_bnds = self._box(vol_bnds, "to_dense")
+        dense = TSDFVolume(vol_bnds, self._voxel_size, device=self.device)
         dims = [int(d) for d in dense._vol_dim]
         if min(dims) > 0:
             tsdf, weight, color = dense.get_volume_tensors()
@@ -380,6 +396,87 @@ class SparseTSDFVolume(_FrameInputs):
                     self._counters.data_ptr(), (ctypes.c_int * 3)(*[int(v) for v in k]), dims[0], dims[1], dims[2],
                     tsdf.data_ptr(), weight.data_ptr(), color.data_ptr(), _stream()), "tsdf_sparse_export")
         return dense
+
+    # ---- mesh and rendering on the blocks (no dense box) ----------------------------------------------------------------
+    def _view_box(self, vol_bnds, what):
+        """_box plus the box's grid as TSDFVolume(vol_bnds) computes it: (n, k as a ctypes int64[3], dims, float32 origin as
+        a ctypes float[3])."""
+        n, k, vol_bnds = self._box(vol_bnds, what)
+        dims = np.ceil((vol_bnds[:, 1] - vol_bnds[:, 0]) / self._voxel_size).astype(int)          # TSDFVolume's (:50, :52)
+        origin = vol_bnds[:, 0].astype(np.float32)
+        if np.any(dims >= 2 ** 31) or float(np.prod(np.maximum(dims, 0).astype(np.float64))) >= 2.0 ** 61:
+            raise ValueError("SparseTSDFVolume.%s: a box of %s voxels is too large (each dimension < 2^31, at most 2^61 voxels)"
+                             % (what, dims.tolist()))
+        return (n, (ctypes.c_longlong * 3)(*[int(v) for v in k]), [int(d) for d in dims],
+                (ctypes.c_float * 3)(*[float(v) for v in origin]))
+
+    def _state(self):
+        return (self._keys.data_ptr(), self._slots.data_ptr(), int(self._keys.numel()), self._coords.data_ptr(), self.capacity,
+                self._counters.data_ptr())
+
+    def get_mesh_tensors(self, vol_bnds=None):
+        """Marching cubes over vol_bnds (to_dense's box, by default the allocated blocks' bounding box) on the blocks: exactly
+        to_dense(vol_bnds).get_mesh_tensors() -- the same vertices, faces, normals and colours in the same order -- without the
+        dense box.  Scratch and outputs scale with the allocated blocks and the mesh.  Synchronises to read the block count and,
+        as TSDFVolume's, once between the count and the extract launches."""
+        n, k, dims, origin = self._view_box(vol_bnds, "get_mesh")
+        dev = self.device
+        with self._device_scope():
+            if n == 0 or min(dims) < 2:
+                return (torch.empty((0, 3), dtype=torch.float32, device=dev), torch.empty((0, 3), dtype=torch.int32, device=dev),
+                        torch.empty((0, 3), dtype=torch.float32, device=dev), torch.empty((0, 3), dtype=torch.uint8, device=dev))
+            nbytes = ctypes.c_longlong(0)
+            N.check(N.lib().dvmvs_tsdf_sparse_mesh_scratch_bytes(n, ctypes.byref(nbytes)), "tsdf_sparse_mesh_scratch_bytes")
+            scratch = torch.empty(max(int(nbytes.value), 16), dtype=torch.uint8, device=dev)
+            stream = _stream()
+            N.check(N.lib().dvmvs_tsdf_sparse_mesh_count(*self._state(), self._tsdf.data_ptr(), n, k, dims[0], dims[1], dims[2],
+                                                         scratch.data_ptr(), scratch.numel(), stream), "tsdf_sparse_mesh_count")
+            n_verts, n_faces = (int(v) for v in scratch[:16].view(torch.int64).cpu())        # the one read between the passes
+            if n_verts >= 2 ** 31 or 3 * n_faces >= 2 ** 31:
+                raise RuntimeError("SparseTSDFVolume.get_mesh: a mesh of %d vertices and %d faces exceeds the int32 indices"
+                                   % (n_verts, n_faces))
+            verts = torch.empty((n_verts, 3), dtype=torch.float32, device=dev)
+            norms = torch.empty((n_verts, 3), dtype=torch.float32, device=dev)
+            colors = torch.empty((n_verts, 3), dtype=torch.uint8, device=dev)
+            faces = torch.empty((n_faces, 3), dtype=torch.int32, device=dev)
+            keys = torch.empty(max(n_verts + 3 * n_faces, 1), dtype=torch.int64, device=dev)
+            N.check(N.lib().dvmvs_tsdf_sparse_mesh_extract(
+                *self._state(), self._tsdf.data_ptr(), self._color.data_ptr(), n, k, dims[0], dims[1], dims[2], origin,
+                self._voxel_size, scratch.data_ptr(), scratch.numel(), n_verts, n_faces, keys.data_ptr(), verts.data_ptr(),
+                faces.data_ptr(), norms.data_ptr(), colors.data_ptr(), stream), "tsdf_sparse_mesh_extract")
+        return verts, faces, norms, colors
+
+    def get_mesh(self, vol_bnds=None):
+        """get_mesh_tensors copied to the host: (verts, faces, norms, colors) numpy arrays, as TSDFVolume.get_mesh."""
+        return tuple(t.cpu().numpy() for t in self.get_mesh_tensors(vol_bnds))
+
+    def get_point_cloud(self, vol_bnds=None):
+        """as TSDFVolume.get_point_cloud: (V,6) vertices and colours."""
+        verts, _, _, colors = self.get_mesh(vol_bnds)
+        return np.hstack([verts, colors])
+
+    def render_tensors(self, cam_intr, cam_poses, height, width, vol_bnds=None):
+        """Ray-cast over vol_bnds (to_dense's box, by default the allocated blocks' bounding box) on the blocks: exactly
+        to_dense(vol_bnds).render_tensors(cam_intr, cam_poses, height, width) -- TSDFVolume.render_tensors' arguments, types,
+        shapes and errors -- without the dense box.  One launch for all views, enqueued on torch's current stream;
+        synchronises once, to read the block count."""
+        with self._device_scope():
+            _, k, dims, origin = self._view_box(vol_bnds, "render")
+            views, n, single, height, width = self._views(cam_intr, cam_poses, height, width)
+            depth = torch.empty((n, height, width), dtype=torch.float32, device=self.device)
+            normals = torch.empty((n, height, width, 3), dtype=torch.float32, device=self.device)
+            colors = torch.empty((n, height, width, 3), dtype=torch.uint8, device=self.device)
+            N.check(N.lib().dvmvs_tsdf_sparse_raycast(
+                *self._state(), self._tsdf.data_ptr(), self._color.data_ptr(), k, dims[0], dims[1], dims[2], origin,
+                self._voxel_size, self._trunc_margin, views.data_ptr(), n, height, width, depth.data_ptr(), normals.data_ptr(),
+                colors.data_ptr(), _stream()), "tsdf_sparse_raycast")
+        if single:
+            return depth[0], normals[0], colors[0]
+        return depth, normals, colors
+
+    def render(self, cam_intr, cam_poses, height, width, vol_bnds=None):
+        """render_tensors copied to the host: (depth, normals, colors) numpy arrays."""
+        return tuple(t.cpu().numpy() for t in self.render_tensors(cam_intr, cam_poses, height, width, vol_bnds))
 
 
 class TSDFFusion(object):
