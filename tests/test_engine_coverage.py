@@ -1,9 +1,11 @@
 """Every native entry point bench.py's default engine launches is covered by an fp64 reference test, and the fp32 CUDA-core, staging
-and geometry calls of the engine pass those references on the engine's own buffers.
+and geometry calls of the engine pass those references on the engine's own buffers; the same at the lookahead engine
+configurations of tools/engine_record.py's ENGINE_POINTS.
 
 ENTRY_TESTS maps each dvmvs_* entry point (and each branch of dvmvs_conv2d) to the test that checks it against fp64; an entry point
 the engine starts launching without one fails test_engine_entry_points_are_covered.  An entry point mapped to the replay test below
-counts as covered at an operating point of bench.py only if that point's replay reaches it."""
+counts as covered at an operating point of bench.py only if that point's replay reaches it.  The tests named here run over
+bench.py's points; ENGINE_POINT_TESTS names their counterparts over ENGINE_POINTS, which run the same replay code."""
 import importlib
 
 import numpy as np
@@ -50,6 +52,14 @@ for _k in (1, 3, 5):
             ENTRY_TESTS["dvmvs_conv2d " + _b] = _CONV_UNIT if _b in UNIT_DIRECT else _REPLAY
 HOST_ONLY = {"dvmvs_conv2d_tc_ksplit", "dvmvs_kernel_launch_count", "dvmvs_last_error_string", "dvmvs_abi_version",
              "dvmvs_set_programmatic_launch"}      # queries and switches: they launch no kernel
+ENGINE_POINT_TESTS = {
+    "tests.test_tc_reference::test_every_benchmark_layer_vs_fp64_reference": "tests.test_tc_reference::test_every_engine_point_layer_vs_fp64_reference",
+    "tests.test_sweep_reference::test_sweep_of_the_benchmarked_engine_vs_fp64_reference":
+        "tests.test_sweep_reference::test_sweep_of_each_engine_point_vs_fp64_reference",
+    _REPLAY: "tests.test_engine_coverage::test_engine_point_calls_replayed_vs_fp64_reference",
+}
+# what only fusionnet's recurrent stage launches (hidden-state warp, depth re-projection, ConvLSTM gates): pairnet launches none of it
+RECURRENT_ENTRY_POINTS = ("dvmvs_hidden_warp", "dvmvs_depth_reproject", "dvmvs_lstm_gates", "dvmvs_lstm_gates_parts")
 
 OPS_REPLAYED = ("stem_conv", "dwconv2d", "split_planes", "concat_planes", "split_blocked", "conv2d", "upsample2x", "hidden_warp", "depth_reproject")
 OP_ENTRY = {"stem_conv": "dvmvs_stem_conv", "dwconv2d": "dvmvs_dwconv2d", "split_planes": "dvmvs_split_planes", "concat_planes": "dvmvs_split_planes",
@@ -63,6 +73,11 @@ def _point_params(with_sizes=()):
     from tools.engine_record import POINTS
     return ([pytest.param("value", None, None, id="256-256")] + [pytest.param("value", h, w, id="%d-%d" % (h, w)) for h, w in with_sizes] +
             [pytest.param(p, None, None, id=p) for p in POINTS if p != "value"])
+
+
+def _engine_point_params():
+    from tools.engine_record import ENGINE_POINTS
+    return list(ENGINE_POINTS)
 
 
 @pytest.fixture(autouse=True)
@@ -86,9 +101,10 @@ def uncovered(recorded):
 
 
 def test_coverage_map_names_existing_tests():
-    for entry, test in ENTRY_TESTS.items():
+    for entry, test in list(ENTRY_TESTS.items()) + list(ENGINE_POINT_TESTS.items()):
         mod, fn = test.split("::")
         assert callable(getattr(importlib.import_module(mod), fn, None)), "%s: %s does not exist" % (entry, test)
+    assert set(ENGINE_POINT_TESTS) <= set(ENTRY_TESTS.values())
 
 
 def test_unit_direct_branches_are_reached():
@@ -143,19 +159,34 @@ def test_engine_entry_points_are_covered():
     _each_point(_entry_points_at)
 
 
+@pytest.mark.parametrize("point", _engine_point_params())
+def test_engine_point_entry_points_are_covered(point):
+    """test_engine_entry_points_are_covered at a lookahead engine configuration of tools/engine_record.py's ENGINE_POINTS"""
+    _entry_points_at(point)
+    torch.cuda.empty_cache()
+
+
 def _entry_points_at(point):
-    from tools.engine_record import engine_calls
+    from tools.engine_record import ENGINE_POINTS, engine_calls
     print("\n" + point)
     native = {}
-    _, calls = engine_calls(OPS_REPLAYED, point=point, native=native)
+    mods, calls = engine_calls(OPS_REPLAYED, point=point, native=native)
     reached = replayed_entry_points(calls)
     for k in sorted(native):
         test = ENTRY_TESTS.get(k, "host only" if k in HOST_ONLY else "NOT COVERED")
-        print("%-40s x%-5d %s%s" % (k, native[k], test, " (NOT REPLAYED HERE)" if test == _REPLAY and k not in reached else ""))
+        if point in ENGINE_POINTS:
+            test = ENGINE_POINT_TESTS.get(test, test)
+        replay = test in (_REPLAY, ENGINE_POINT_TESTS[_REPLAY])
+        print("%-40s x%-5d %s%s" % (k, native[k], test, " (NOT REPLAYED HERE)" if replay and k not in reached else ""))
     assert not uncovered(native), "%s: the engine launches entry points no fp64 test covers: %s" % (point, uncovered(native))
     assert not uncovered_at(native, reached), "%s: launched, mapped to the replay, but not replayed at this point: %s" % (point, uncovered_at(native, reached))
-    for must in ("dvmvs_stem_conv", "dvmvs_split_blocked", "dvmvs_hidden_warp", "dvmvs_depth_reproject", "dvmvs_conv2d", "dvmvs_conv2d_tc"):
+    recurrent = "lstm" in mods
+    for must in ("dvmvs_stem_conv", "dvmvs_split_blocked", "dvmvs_conv2d", "dvmvs_conv2d_tc") + (
+            ("dvmvs_hidden_warp", "dvmvs_depth_reproject") if recurrent else ()):
         assert must in native, "%s: the engine no longer calls %s: update ENTRY_TESTS and this list" % (point, must)
+    if not recurrent:
+        launched = [k for k in RECURRENT_ENTRY_POINTS if k in native]
+        assert not launched, "%s: pairnet launches recurrent-stage entry points %s" % (point, launched)
     dropped = dict(ENTRY_TESTS)
     dropped.pop("dvmvs_stem_conv")           # the check is not vacuous: an entry point missing from the map is reported
     assert [k for k in native if k not in dropped and k not in HOST_ONLY] == ["dvmvs_stem_conv"]
@@ -295,18 +326,17 @@ def _row_motion(synth, B):
     return prev, cur
 
 
-@pytest.mark.parametrize("point,height,width", _point_params(with_sizes=[(320, 256)]))
-def test_engine_calls_replayed_vs_fp64_reference(point, height, width, synth):
-    """Records every stem, depthwise, staging, dvmvs_conv2d (depth head), upsampling, hidden-warp and re-projection call of the engine
-    bench.py runs at this operating point, and replays each on its buffers against the fp64 reference, on the batch rows
-    tools.engine_record.batch_rows picks; the warp and the re-projection once more with a different camera motion in every batch
-    row (priming repeats one frame: the recorded poses are an identity motion).  Checks the trunk batch of the point."""
-    import time
-    from tools.engine_record import batch_rows, engine_calls, point_config, trunk_batch
-    t0 = time.perf_counter()
+def _replay_engine_calls(point, synth, height=None, width=None):
+    """Records every stem, depthwise, staging, dvmvs_conv2d (depth head), upsampling, hidden-warp and re-projection call of the
+    engine of this operating point (tools/engine_record.py POINTS or ENGINE_POINTS), and replays each on its buffers against the
+    fp64 reference, on the batch rows tools.engine_record.batch_rows picks; the warp and the re-projection once more with a
+    different camera motion in every batch row (priming repeats one frame: the recorded poses are an identity motion).  One line
+    per call.  Returns (cfg, calls replayed per op, stem batches, batches of the dvmvs_conv2d calls of the decoder's layers)."""
+    from tools.engine_record import batch_rows, engine_calls, layer_names, point_config
     cfg = point_config(point, height, width)
     mods, calls = engine_calls(OPS_REPLAYED, point=point, height=height, width=width)
-    seen, stem_batch = {}, set()
+    names = layer_names(mods)
+    seen, stem_batch, head_batch = {}, set(), set()
     print()
     for key, (args, kw, lay, on_rec) in calls.items():
         name = key[0]
@@ -320,6 +350,8 @@ def test_engine_calls_replayed_vs_fp64_reference(point, height, width, synth):
         seen[name] = seen.get(name, 0) + 1
         if name == "stem_conv":
             stem_batch.add(B)
+        if name == "conv2d" and names.get(id(lay), "").startswith("cvd"):
+            head_batch.add(B)
         print("%-16s %-60s B=%-3d rows=%d %s %s" % (name, str(key[1:])[:60], B, len(rows), "err/bound %.3f" % worst if worst is not None else "", note))
     for key, (args, kw, _, _) in calls.items():
         if key[0] not in ("hidden_warp", "depth_reproject"):
@@ -333,8 +365,40 @@ def test_engine_calls_replayed_vs_fp64_reference(point, height, width, synth):
         else:
             n = _check_reproject("depth_reproject, a motion per row", args, rows, prev=prev, cur=cur)
             print("depth_reproject, a motion per row  B=%d ambiguous sources %d" % (B, n))
+    return cfg, seen, stem_batch, head_batch
+
+
+@pytest.mark.parametrize("point,height,width", _point_params(with_sizes=[(320, 256)]))
+def test_engine_calls_replayed_vs_fp64_reference(point, height, width, synth):
+    """Every stem, depthwise, staging, dvmvs_conv2d (depth head), upsampling, hidden-warp and re-projection call of the engine
+    bench.py runs at this operating point, replayed against the fp64 reference (_replay_engine_calls).  Checks the trunk batch of
+    the point."""
+    import time
+    from tools.engine_record import trunk_batch
+    t0 = time.perf_counter()
+    cfg, seen, stem_batch, _ = _replay_engine_calls(point, synth, height, width)
     print("%s %dx%d B=%d: replayed %s; stem batch %s; %.1f s" % (point, cfg["height"], cfg["width"], cfg["batch"], seen, sorted(stem_batch),
                                                               time.perf_counter() - t0))
     for must in ("stem_conv", "split_blocked", "conv2d", "hidden_warp", "depth_reproject"):
         assert seen.get(must), "%s: the engine made no %s call" % (point, must)
     assert stem_batch == {trunk_batch(cfg)}, "%s: stem batch %s, expected %d" % (point, sorted(stem_batch), trunk_batch(cfg))
+
+
+@pytest.mark.parametrize("point", _engine_point_params())
+def test_engine_point_calls_replayed_vs_fp64_reference(point, synth):
+    """test_engine_calls_replayed_vs_fp64_reference at a lookahead engine configuration of tools/engine_record.py's ENGINE_POINTS.
+    Checks the trunk batches, the batch of the decoder's depth heads, and that pairnet runs no hidden warp or re-projection."""
+    import time
+    from tools.engine_record import decoder_batch, trunk_batches
+    t0 = time.perf_counter()
+    cfg, seen, stem_batch, head_batch = _replay_engine_calls(point, synth)
+    print("%s %dx%d B=%d lookahead=%d cache=%d: replayed %s; stem batch %s; depth-head batch %s; %.1f s" % (
+        point, cfg["height"], cfg["width"], cfg["batch"], cfg["lookahead"], cfg["feature_cache"], seen, sorted(stem_batch), sorted(head_batch),
+        time.perf_counter() - t0))
+    recurrent = ("hidden_warp", "depth_reproject")
+    for must in ("stem_conv", "split_blocked", "conv2d") + (recurrent if cfg["engine"] != "pairnet" else ()):
+        assert must in seen, "%s: the engine made no %s call" % (point, must)
+    if cfg["engine"] == "pairnet":
+        assert not set(recurrent) & set(seen), "%s: pairnet made recurrent-stage calls %s" % (point, seen)
+    assert stem_batch == trunk_batches(cfg), "%s: stem batch %s, expected %s" % (point, sorted(stem_batch), sorted(trunk_batches(cfg)))
+    assert head_batch == {decoder_batch(cfg)}, "%s: depth-head (cvd.*) batch %s, expected %d" % (point, sorted(head_batch), decoder_batch(cfg))

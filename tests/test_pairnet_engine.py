@@ -80,21 +80,27 @@ def _clip_args(clip, k):
 
 
 # ------------------------------------------------------------------------------------------------ accuracy
-@pytest.mark.parametrize("B", [1, 2])
-@pytest.mark.parametrize("backend,terms,bound", [("fp32", 3, 1e-5), ("tc", 3, 1e-5), ("tc", 1, 1e-4)])
-def test_pairnet_engine_matches_eager_keyframe(oracle, synth, backend, terms, bound, B):
-    """Two synthetic clips back to back (7 + 4 keyframes in groups of 3: the last group incomplete) against eager keyframe()
-    with pairnet modules on the same backend.  Not bit for bit: the split-K choice of a few convolutions depends on the batch."""
+# backend, terms, bound, B, (H, W, D, M), lookahead; the last one is c1 at pairnet_bench.py's largest group (8 clips x lookahead 8)
+EAGER_CASES = [pytest.param(backend, terms, bound, B, (64, 96, 64, 2), 3, id="%s-%d-%g-%d" % (backend, terms, bound, B))
+               for backend, terms, bound in [("fp32", 3, 1e-5), ("tc", 3, 1e-5), ("tc", 1, 1e-4)] for B in (1, 2)]
+EAGER_CASES.append(pytest.param("tc", 1, 1e-4, 8, (128, 128, 32, 1), 8, id="c1-tc-1-0.0001-8-lookahead8"))
+
+
+@pytest.mark.parametrize("backend,terms,bound,B,shape,T", EAGER_CASES)
+def test_pairnet_engine_matches_eager_keyframe(oracle, synth, backend, terms, bound, B, shape, T):
+    """Two synthetic clips back to back (7 + 4 keyframes in groups of T: the last group incomplete) against eager keyframe()
+    with pairnet modules on the same backend: every keyframe's rows of the group read its own inputs and land in its own
+    output.  Not bit for bit: the split-K choice of a few convolutions depends on the batch."""
     from dvmvs import _ops as ops
     from dvmvs import pipeline
-    H, W, D, M = 64, 96, 64, 2
+    H, W, D, M = shape
     old = ops.conv_backend()
     ops.set_conv_backend(backend, terms=terms, stride2=True)
     try:
         with torch.no_grad():
             mods, _ = _pairnet_modules(oracle, synth, D)
             frames = _frames(synth, B, 7, H, W, M) + _frames_of_seed(synth, 20, B, 4, H, W, M)
-            eng = _engine(mods, B, H, W, M, D)
+            eng = _engine(mods, B, H, W, M, D, T=T)
             eng.prime(*frames[0])
             expected, got = [], []
             for i, f in enumerate(frames):
@@ -106,7 +112,8 @@ def test_pairnet_engine_matches_eager_keyframe(oracle, synth, backend, terms, bo
             eng.synchronize()
         assert B == 1 or not torch.equal(expected[-1][0], expected[-1][-1]), "the batch rows hold the same clip"
         errs = [float((o - e).abs().sum() / e.abs().sum()) for (_, o), e in zip(got, expected)]
-        print("pairnet lookahead engine vs eager keyframe (%s, %d terms, B=%d): rel-L1 per keyframe" % (backend, terms, B),
+        print("pairnet lookahead engine vs eager keyframe (%s, %d terms, B=%d, %dx%d D=%d M=%d, lookahead %d): rel-L1 per keyframe"
+              % (backend, terms, B, H, W, D, M, T),
               ["%.1e" % e for e in errs])
         assert max(errs) <= bound, errs
         assert torch.equal(eng.depth_of(got[-1][0]), got[-1][1])

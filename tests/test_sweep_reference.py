@@ -340,25 +340,24 @@ def test_sweep_of_the_benchmarked_engine_vs_fp64_reference(ops):
     assert not failed, "\n".join("%s: %s" % kv for kv in failed.items())
 
 
-def _engine_sweep_at(ops, point):
-    """the plane_sweep_tc launch of the engine bench.py runs at this operating point, recorded while it runs as bench.py runs it
-    and replayed on its own buffers: the FPN features it really sweeps, under the bound of the point's terms, on the batch rows
-    tools.engine_record.batch_rows picks.  Checks the sweep's batch, D, M and terms against the point's configuration."""
+def _engine_sweep_at(ops, point, engine=None):
+    """the plane_sweep_tc launch of the engine of this operating point (tools/engine_record.py POINTS or ENGINE_POINTS), recorded
+    while it runs as its benchmark runs it and replayed on its own buffers: the FPN features it really sweeps, under the bound of
+    the point's terms, on the batch rows tools.engine_record.batch_rows picks.  Checks the sweep's batch, D, M and terms against
+    the point's configuration.  Returns the recorded call (args, kwargs); engine: a list the driven engine is appended to."""
     import time
-    from tools.engine_record import batch_rows, engine_calls, point_config
+    from tools.engine_record import batch_rows, engine_calls, group_batch, point_config
     t0 = time.perf_counter()
     cfg = point_config(point)
-    _, calls = engine_calls(("plane_sweep_tc",), point=point)
+    _, calls = engine_calls(("plane_sweep_tc",), point=point, engine=engine)
     sweeps = [v for k, v in calls.items() if k[0] == "plane_sweep_tc"]
     assert len(sweeps) == 1, "%s: the engine launched %d plane_sweep_tc call sites" % (point, len(sweeps))
     for args, kw, _, _ in sweeps:
         ref_pair, meas_pairs, pose1, pose2s, K, mn, mx, D = args[:8]
         terms = kw.get("terms", 3)
         B, h, w, _ = ref_pair[0].shape
-        expect_B = cfg["batch"] * (cfg["lookahead"] if cfg["engine"] == "lookahead" else 1)
-        assert (B, D, len(pose2s), terms) == (expect_B, cfg["n_depth_levels"], cfg["n_measurement_frames"], cfg["terms"]), (
-            "%s: sweep B, D, M, terms = %s, expected %s" % (point, (B, D, len(pose2s), terms),
-                                                          (expect_B, cfg["n_depth_levels"], cfg["n_measurement_frames"], cfg["terms"])))
+        expect = (group_batch(cfg), cfg["n_depth_levels"], cfg["n_measurement_frames"], cfg["terms"])
+        assert (B, D, len(pose2s), terms) == expect, "%s: sweep B, D, M, terms = %s, expected %s" % (point, (B, D, len(pose2s), terms), expect)
         rows = torch.tensor(batch_rows(B), device=DEV)
         sel = lambda t: t.index_select(0, rows)
         pl = lambda p: (sel(p[0]), sel(p[1]) if terms == 3 else None)
@@ -378,3 +377,41 @@ def _engine_sweep_at(ops, point):
                   time.perf_counter() - t0))
         assert acc <= C_ACC / 8
         assert ref.smax < FP16_MAX / 8, "the engine's correlations come within 8x of the fp16 range of the 1-term S"
+    return sweeps[0][:2]
+
+
+def _engine_point_params():
+    from tools.engine_record import ENGINE_POINTS
+    return list(ENGINE_POINTS)
+
+
+@pytest.mark.parametrize("point", _engine_point_params())
+def test_sweep_of_each_engine_point_vs_fp64_reference(ops, point):
+    """_engine_sweep_at at a lookahead engine configuration of tools/engine_record.py's ENGINE_POINTS.  With a feature cache the
+    measurement operands are not the feature pyramid's: the sweep stage gathers every keyframe's measurement features from the
+    cache's ring (fp32 rows) and stages them as fp16 (hi, lo) planes.  So for those points: each keyframe's B rows of every
+    measurement operand are, bit for bit, the staging of one ring entry other than the sink -- an entry the engine filled."""
+    from tools.engine_record import point_config
+    cfg = point_config(point)
+    engine = []
+    args, kw = _engine_sweep_at(ops, point, engine)
+    (eng,) = engine
+    assert (eng.cache is not None) == bool(cfg["feature_cache"]), "%s: engine built with cache %s" % (point, eng.cache)
+    if eng.cache is None:
+        return
+    from tests.tc_reference import check_live
+    B, terms, meas_pairs = cfg["batch"], kw.get("terms", 3), args[1]
+    ring = eng.cache.ring[:eng.cache.capacity]
+    with torch.no_grad():
+        staged = ops.split_planes(ring.reshape((-1,) + tuple(ring.shape[2:]))).view((2,) + tuple(ring.shape))     # (2, entries, B, h, w, 32)
+        torch.cuda.synchronize()
+    matched = []
+    for m, (hi, lo) in enumerate(meas_pairs):
+        for j in range(hi.shape[0] // B):
+            rows = slice(j * B, (j + 1) * B)
+            check_live("%s measurement %d keyframe %d" % (point, m, j), hi[rows])
+            same = [e for e in range(ring.shape[0]) if torch.equal(staged[0, e], hi[rows]) and (terms == 1 or torch.equal(staged[1, e], lo[rows]))]
+            assert same, "%s: measurement operand %d, keyframe %d of the group is the staging of no ring entry" % (point, m, j)
+            matched.append(same[0])
+    print("%s: the sweep's %d measurement operands x %d keyframes are stagings of ring entries (first match each) %s" % (
+        point, len(meas_pairs), meas_pairs[0][0].shape[0] // B, matched))

@@ -51,7 +51,7 @@ def _fill_lo(ptr, n):
 
 class NativeSpy:
     """Wraps the library's dvmvs_conv2d_tc / dvmvs_conv2d_halo while active: records the split count (dvmvs_conv2d_tc_ksplit on
-    the same descriptor), the output tile, block_n, terms and batch of every conv2d_tc launch, and fills the lo plane of every fp16 output of a
+    the same descriptor), the output tile, block_n, terms, batch and output map of every conv2d_tc launch, and fills the lo plane of every fp16 output of a
     hi-plane-only launch with SENTINEL first, so that a test can tell the plane was left alone."""
 
     def __enter__(self):
@@ -65,7 +65,7 @@ class NativeSpy:
             pad = (d.ksize - 1) // 2
             Ho, Wo = (d.Hin + 2 * pad - d.ksize) // d.stride + 1, (d.Win + 2 * pad - d.ksize) // d.stride + 1
             self.tc.append({"ksplit": int(L.dvmvs_conv2d_tc_ksplit(dref)), "tile": "8x16" if (Wo <= 8 and Ho > 8) else "16x8",
-                            "block_n": int(d.block_n), "terms": int(d.terms), "B": int(d.B)})
+                            "block_n": int(d.block_n), "terms": int(d.terms), "B": int(d.B), "Ho": Ho, "Wo": Wo})
             if d.out_hi_only:
                 n = d.B * Ho * Wo * d.Cout
                 _fill_lo(d.out_planes, n)
@@ -472,25 +472,20 @@ def _point_params():
             [pytest.param(p, None, None, id=p) for p in POINTS])
 
 
-@pytest.mark.parametrize("point,height,width", _point_params())
-def test_every_benchmark_layer_vs_fp64_reference(ops, point, height, width):
+def _replay_engine_layers(point, height=None, width=None):
     """Records every conv2d_tc, conv2d_halo, expand_dwconv and ConvLSTM gate call (deferred pair or plain epilogue) of the engine
-    bench.py runs at this operating point (seed-7 weights, the point's operand terms and batch, clip b in batch row b), and replays
-    each on its recorded operands against the fp64 reference, on the batch rows tools.engine_record.batch_rows picks.  One line
-    per layer; a failure names the layer.  Then checks the facts that make the point differ from the headline (batch, split
-    counts, block_n, gate path and instantiation, terms, aggregator0's cost-volume channels)."""
-    import time
-    from tools.engine_record import batch_rows, engine_calls, layer_names, point_config, trunk_batch
-    t0 = time.perf_counter()
+    of this operating point (tools/engine_record.py POINTS or ENGINE_POINTS: seed-7 weights, the point's operand terms, batch,
+    lookahead and feature cache, clip b in batch row b), and replays each on its recorded operands against the fp64 reference,
+    on the batch rows tools.engine_record.batch_rows picks.  One line per layer; a failure names the point, the layer, the
+    stage and the input shape.  Returns (cfg, mods, records, seen): per replayed call its layer (name and ConvLayer), path,
+    input B,H,W, conv2d_tc launch facts, operand terms, gate instantiation, stream and worst err / bound; calls per kind."""
+    from tools.engine_record import batch_rows, engine_calls, last_stage, layer_names, point_config
     cfg = point_config(point, height, width)
     mods, calls = engine_calls(("conv2d_tc", "conv2d_halo", "expand_dwconv", "lstm_gates"), point=point, height=height, width=width)
     names = layer_names(mods)
-    gate_layer = mods["lstm"].lstm_cell.packed()[1]             # conv(W[:, Cin:], h): the gate convolution on the recurrent state
-    agg0 = mods["cve"].packed()[0]
     gates_calls = [v for k, v in calls.items() if k[0] == "lstm_gates" and k[2]]
     seen = {"conv2d_tc": 0, "conv2d_halo": 0, "expand_dwconv": 0, "deferred": 0, "lstm_gates": 0}
-    tiles, worst_all, acc_all = set(), 0.0, 0.0
-    trunk, terms_seen, tc_launches, gate, agg0_seen = set(), set(), [], {}, False
+    records = []
     print()
     for key, (args, kw, lay, on_rec) in calls.items():
         kind = key[0]
@@ -505,8 +500,9 @@ def test_every_benchmark_layer_vs_fp64_reference(ops, point, height, width):
             path, shape = "gates", tuple(args[1].shape[:3])
         else:
             path, shape = "expand_dw", tuple(args[0].get_planes().shape[1:4])
+        stage = last_stage(cfg) if on_rec else None
         rows = torch.tensor(batch_rows(shape[0]), device=DEV)
-        launch, acc, extra = {}, 0.0, ""
+        launch, acc, extra, terms, gates = {}, 0.0, "", None, None
         try:
             with NativeSpy() as spy:
                 if path == "tc deferred+gates":
@@ -514,39 +510,51 @@ def test_every_benchmark_layer_vs_fp64_reference(ops, point, height, width):
                     launch, worst, acc = _replay_deferred(args, kw, lay, gates_calls[0], spy, rows)
                     assert launch["ksplit"] > 1
                     seen["deferred"] += 1
-                    extra = " gates=<%d,%d>" % launch["gates"]
+                    gates = launch["gates"]
                 elif path == "tc":
                     launch, worst, acc = _replay_tc(args, kw, lay, spy, rows)
                 elif path == "gates":
-                    inst, worst = _replay_gates(args, rows)
-                    gate["plain"] = inst
-                    extra = " gates=<%d,%d>" % inst
+                    gates, worst = _replay_gates(args, rows)
                 elif path == "halo":
                     worst, acc = _replay_halo(args, kw, lay, rows)
+                    terms = kw["terms"]
                 else:
-                    worst, _, expand_terms = _replay_expand(args, kw, rows)
+                    worst, _, terms = _replay_expand(args, kw, rows)
         except AssertionError as e:
-            raise AssertionError("%s: layer %s (%s%s, input B,H,W=%s): %s" % (point, layer, path, ", recurrent stage" if on_rec else "", shape, e)) from None
+            raise AssertionError("%s: layer %s (%s%s, input B,H,W=%s): %s" % (point, layer, path, ", " + stage if stage else "", shape, e)) from None
         seen[kind] += 1
-        if path.startswith("tc"):
-            tiles.add(launch["tile"])
-            tc_launches.append((layer, launch))
-            terms_seen.add(launch["terms"])
-            if lay is gate_layer:
-                gate["conv"] = launch
-        elif path == "halo":
-            terms_seen.add(kw["terms"])
-        elif path == "expand_dw":
-            terms_seen.add(expand_terms)
-        if layer.startswith("fe"):
-            trunk.add(shape[0])
-        if lay is agg0:
-            agg0_seen = True
-            assert lay.src_channels == [32, cfg["n_depth_levels"]], "%s: aggregator0 reads %s" % (point, lay.src_channels)
-        worst_all, acc_all = max(worst_all, worst), max(acc_all, acc)
+        if launch:
+            terms = launch["terms"]
+        if gates is not None:
+            extra = " gates=<%d,%d>" % gates
+        records.append(dict(layer=layer, lay=lay, path=path, shape=shape, launch=launch, terms=terms, gates=gates, on_rec=on_rec,
+                            worst=worst, acc=acc))
         facts = ("ksplit=%d block_n=%-3d terms=%d tile=%-4s" % (launch["ksplit"], launch["block_n"], launch["terms"], launch["tile"])
                  if launch else "%-34s" % "")
-        _report("%-34s %-18s B,H,W=%-15s %s rows=%d err/bound %.3f  err/(u n S) %.3f%s" % (layer, path, shape, facts, len(rows), worst, acc, extra))
+        _report("%-34s %-18s B,H,W=%-15s %s rows=%d err/bound %.3f  err/(u n S) %.3f%s%s" % (layer, path, shape, facts, len(rows), worst, acc,
+                                                                                            extra, " [%s]" % stage if stage else ""))
+    return cfg, mods, records, seen
+
+
+@pytest.mark.parametrize("point,height,width", _point_params())
+def test_every_benchmark_layer_vs_fp64_reference(ops, point, height, width):
+    """Every conv2d_tc, conv2d_halo, expand_dwconv and ConvLSTM gate call of the engine bench.py runs at this operating point,
+    replayed against the fp64 reference (_replay_engine_layers).  Then checks the facts that make the point differ from the
+    headline (batch, split counts, block_n, gate path and instantiation, terms, aggregator0's cost-volume channels)."""
+    import time
+    from tools.engine_record import trunk_batch
+    t0 = time.perf_counter()
+    cfg, mods, records, seen = _replay_engine_layers(point, height, width)
+    gate_layer = mods["lstm"].lstm_cell.packed()[1]             # conv(W[:, Cin:], h): the gate convolution on the recurrent state
+    agg0 = mods["cve"].packed()[0]
+    tc_launches = [(r["layer"], r["launch"]) for r in records if r["launch"]]
+    tiles = {launch["tile"] for _, launch in tc_launches}
+    terms_seen = {r["terms"] for r in records if r["terms"] is not None}
+    trunk = {r["shape"][0] for r in records if r["layer"].startswith("fe")}
+    gate = {"conv": r["launch"] for r in records if r["lay"] is gate_layer}
+    gate.update({"plain": r["gates"] for r in records if r["path"] == "gates"})
+    agg0_seen = [r["lay"].src_channels for r in records if r["lay"] is agg0]
+    worst_all, acc_all = max(r["worst"] for r in records), max(r["acc"] for r in records)
     deferred = seen["deferred"] > 0
     _report("%s %dx%d B=%d terms=%d: %s; trunk batch %s; gate %s; worst err/bound %.3f, worst err/(u n S) %.3f (C_ACC = %g); %.1f s" % (
         point, cfg["height"], cfg["width"], cfg["batch"], cfg["terms"], seen, sorted(trunk),
@@ -555,6 +563,7 @@ def test_every_benchmark_layer_vs_fp64_reference(ops, point, height, width):
     # what makes this point this point
     assert all(seen[k] > 0 for k in ("conv2d_tc", "conv2d_halo", "expand_dwconv")), seen
     assert "conv" in gate and agg0_seen, "%s: the gate convolution or aggregator0 was not replayed" % point
+    assert all(c == [32, cfg["n_depth_levels"]] for c in agg0_seen), "%s: aggregator0 reads %s" % (point, agg0_seen)
     assert trunk == {trunk_batch(cfg)}, "%s: trunk batch %s, expected %d" % (point, sorted(trunk), trunk_batch(cfg))
     assert terms_seen == {cfg["terms"]}, "%s: tensor-core calls at terms %s, expected %d" % (point, terms_seen, cfg["terms"])
     assert gate["conv"]["B"] == cfg["batch"]
@@ -570,3 +579,51 @@ def test_every_benchmark_layer_vs_fp64_reference(ops, point, height, width):
         assert not split, "%s: conv2d_tc calls that split: %s" % (point, split)
     if (cfg["height"], cfg["width"]) == (320, 256):
         assert "8x16" in tiles, "the 10x8 bottleneck of a portrait input no longer runs the 8-wide tile"
+
+
+def _engine_point_params():
+    from tools.engine_record import ENGINE_POINTS
+    return list(ENGINE_POINTS)
+
+
+@pytest.mark.parametrize("point", _engine_point_params())
+def test_every_engine_point_layer_vs_fp64_reference(ops, point):
+    """The lookahead engine configurations of tools/engine_record.py's ENGINE_POINTS (LookaheadPairnet at c1 and c2 up to
+    lookahead 8 x batch 8, both lookahead engines with the feature cache): every conv2d_tc, conv2d_halo, expand_dwconv and
+    ConvLSTM gate call replayed against the fp64 reference (_replay_engine_layers).  Then the facts that make the configuration
+    what it is: the trunk batches, the decoder's batch, aggregator0's cost-volume channels, the operand terms, the ConvLSTM
+    gate calls (none in pairnet), and at c1 conv2d_tc launches on the 4x4 maps of the 1/32 level -- at a group of one keyframe
+    with block_n 32 and split over K."""
+    import time
+    from tools.engine_record import decoder_batch, group_batch, trunk_batches
+    t0 = time.perf_counter()
+    cfg, mods, records, seen = _replay_engine_layers(point)
+    agg0 = mods["cve"].packed()[0]
+    trunk = {r["shape"][0] for r in records if r["layer"].startswith("fe")}
+    decoder = {r["shape"][0] for r in records if r["layer"].startswith("cvd")}
+    terms_seen = {r["terms"] for r in records if r["terms"] is not None}
+    agg0_seen = [r["lay"].src_channels for r in records if r["lay"] is agg0]
+    tiny = [r for r in records if r["launch"] and (r["launch"]["Ho"], r["launch"]["Wo"]) == (4, 4)]
+    worst_all, acc_all = max(r["worst"] for r in records), max(r["acc"] for r in records)
+    _report("%s %dx%d D=%d M=%d B=%d lookahead=%d terms=%d cache=%d: %s; trunk batch %s; decoder batch %s; conv2d_tc on 4x4 maps: %d "
+            "(ksplit %s, block_n %s); worst err/bound %.3f, worst err/(u n S) %.3f (C_ACC = %g); %.1f s" % (
+                point, cfg["height"], cfg["width"], cfg["n_depth_levels"], cfg["n_measurement_frames"], cfg["batch"], cfg["lookahead"],
+                cfg["terms"], cfg["feature_cache"], seen, sorted(trunk), sorted(decoder), len(tiny),
+                sorted({r["launch"]["ksplit"] for r in tiny}), sorted({r["launch"]["block_n"] for r in tiny}), worst_all, acc_all, R.C_ACC,
+                time.perf_counter() - t0))
+    assert all(seen[k] > 0 for k in ("conv2d_tc", "conv2d_halo", "expand_dwconv")), seen
+    assert agg0_seen and all(c == [32, cfg["n_depth_levels"]] for c in agg0_seen), "%s: aggregator0 reads %s" % (point, agg0_seen)
+    assert trunk == trunk_batches(cfg), "%s: trunk batch %s, expected %s" % (point, sorted(trunk), sorted(trunk_batches(cfg)))
+    assert decoder == {decoder_batch(cfg)}, "%s: decoder (cvd.*) batch %s, expected %d: %s" % (
+        point, sorted(decoder), decoder_batch(cfg), ["%s %s" % (r["layer"], r["shape"]) for r in records
+                                                     if r["layer"].startswith("cvd") and r["shape"][0] != decoder_batch(cfg)][:4])
+    assert terms_seen == {cfg["terms"]}, "%s: tensor-core calls at terms %s, expected %d" % (point, terms_seen, cfg["terms"])
+    if "lstm" in mods:
+        assert seen["deferred"] + seen["lstm_gates"] == 1, "%s: the ConvLSTM gate epilogue was not replayed (%s)" % (point, seen)
+    else:
+        assert seen["deferred"] == seen["lstm_gates"] == 0, "%s: pairnet recorded ConvLSTM gate calls (%s)" % (point, seen)
+    if (cfg["height"], cfg["width"]) == (128, 128):
+        assert tiny, "%s: no conv2d_tc launch on a 4x4 output map" % point
+        if group_batch(cfg) == 1:
+            assert any(r["launch"]["ksplit"] > 1 for r in tiny), "%s: no 4x4 conv2d_tc launch splits over K" % point
+            assert any(r["launch"]["block_n"] == 32 for r in tiny), "%s: no 4x4 conv2d_tc launch at block_n 32" % point

@@ -1,5 +1,6 @@
-"""Records the calls bench.py's engines make at each operating point bench.py reports (POINTS): used by tools/tc_bench.py to time
-each layer alone and by the fp64 reference tests (tests/test_tc_reference.py, tests/test_engine_coverage.py,
+"""Records the calls the depth engines make at each operating point bench.py reports (POINTS) and at the lookahead engine
+configurations tools/pairnet_bench.py and tools/lookahead_cache_bench.py measure (ENGINE_POINTS): used by tools/tc_bench.py to
+time each layer alone and by the fp64 reference tests (tests/test_tc_reference.py, tests/test_engine_coverage.py,
 tests/test_sweep_reference.py) to check each call on the engine's own buffers, and to list every dvmvs_* entry point of the native
 library the engine launches."""
 import os
@@ -109,12 +110,37 @@ NON_KERNEL_POINTS = {
 }
 
 
+# The lookahead engines at the configurations tools/pairnet_bench.py and tools/lookahead_cache_bench.py measure, beyond bench.py's
+# points: "pairnet" is LookaheadPairnet (pairnet modules: no LSTMFusion; the decoder runs over the whole group), "lookahead" is
+# LookaheadFusionnet.  c1 (128x128, D = 32, M = 1) is the only input size whose 1/32 maps are 4x4 (bench.py's smallest are 8x8);
+# the pairnet group batches (lookahead x batch, up to 64 keyframes and a 192-image trunk) are bench.py's largest or beyond; the
+# feature cache size is lookahead_cache_bench.py's max(30, lookahead x (M + 1)).  (c2, batch 1, lookahead 1), pairnet_bench.py's
+# smallest group at c2, has no row: its maps are 8x8 and larger and its batches those of bench.py's batch-1 points, which the
+# replays run over POINTS; c1's smallest group is the one whose maps and batches no other configuration reaches.
+C1 = dict(height=128, width=128, n_depth_levels=32, n_measurement_frames=1)
+C2 = dict(height=256, width=256, n_depth_levels=64, n_measurement_frames=2)
+C3 = dict(height=256, width=320, n_depth_levels=96, n_measurement_frames=4)
+ENGINE_POINTS = {
+    "pairnet_c1_b1_t1": dict(engine="pairnet", batch=1, lookahead=1, **C1),
+    "pairnet_c1_b1_t8": dict(engine="pairnet", batch=1, lookahead=8, **C1),
+    "pairnet_c1_b8_t8": dict(engine="pairnet", batch=8, lookahead=8, **C1),
+    "pairnet_c1_b1_t8_cache": dict(engine="pairnet", batch=1, lookahead=8, feature_cache=30, **C1),
+    "pairnet_c2_b1_t4": dict(engine="pairnet", batch=1, lookahead=4, **C2),
+    "pairnet_c2_b1_t4_3terms": dict(engine="pairnet", batch=1, lookahead=4, terms=3, **C2),
+    "pairnet_c2_b1_t4_cache": dict(engine="pairnet", batch=1, lookahead=4, feature_cache=30, **C2),
+    "pairnet_c2_b8_t8": dict(engine="pairnet", batch=8, lookahead=8, **C2),
+    "fusionnet_c2_t4_cache": dict(engine="lookahead", batch=1, lookahead=4, feature_cache=30, **C2),
+    "fusionnet_c3_t4_cache": dict(engine="lookahead", batch=1, lookahead=4, feature_cache=30, **C3),
+}
+
+
 def point_config(point="value", height=None, width=None):
-    """the full configuration of an operating point (bench.py's defaults filled in; height / width override the input size)"""
+    """the full configuration of an operating point of POINTS or ENGINE_POINTS (bench.py's defaults filled in; height / width
+    override the input size)"""
     import bench
     cfg = dict(engine="lookahead", batch=1, height=bench.H, width=bench.W, n_depth_levels=bench.D, n_measurement_frames=bench.M, terms=1,
                feature_cache=0, lookahead=4, n_stages=5)
-    cfg.update(POINTS[point])
+    cfg.update(POINTS[point] if point in POINTS else ENGINE_POINTS[point])
     if height is not None:
         cfg["height"] = height
     if width is not None:
@@ -122,14 +148,40 @@ def point_config(point="value", height=None, width=None):
     return cfg
 
 
+def group_batch(cfg):
+    """rows of one launch of the state-independent stages: lookahead x batch keyframes for the lookahead engines, the batch
+    for the others"""
+    return cfg["batch"] * (cfg["lookahead"] if cfg["engine"] in ("lookahead", "pairnet") else 1)
+
+
+def decoder_batch(cfg):
+    """the decoder's batch: pairnet decodes a whole group at once; fusionnet decodes each keyframe on its recurrent stage"""
+    return group_batch(cfg) if cfg["engine"] == "pairnet" else cfg["batch"]
+
+
+def last_stage(cfg):
+    """what the engine's last stream runs: fusionnet's loop-carried (recurrent) stage, pairnet's decoder over the group"""
+    return "decoder stage" if cfg["engine"] == "pairnet" else "recurrent stage"
+
+
 def trunk_batch(cfg):
-    """images per MnasNet trunk launch at this point: reference + measurement frames stacked over the batch (and over the
-    lookahead group), the reference frames alone when the measurement features come from the cache, one image per pass in
-    the script's call sequence"""
+    """images per MnasNet trunk launch of the engine's graphs at this point: reference + measurement frames stacked over the
+    batch (and over the lookahead group), the reference frames alone when the measurement features come from the cache, one
+    image per pass in the script's call sequence"""
     if cfg["engine"] == "script":
         return cfg["batch"]
     per = 1 if cfg["feature_cache"] else cfg["n_measurement_frames"] + 1
-    return per * cfg["batch"] * (cfg["lookahead"] if cfg["engine"] == "lookahead" else 1)
+    return per * group_batch(cfg)
+
+
+def trunk_batches(cfg):
+    """every batch the MnasNet trunk runs at this point: trunk_batch, and for a lookahead engine with a feature cache also the
+    batch itself -- that engine runs the trunk eagerly, at the batch, on each measurement frame that missed the cache (the
+    other engines run their misses at the batch of their graphs)"""
+    batches = {trunk_batch(cfg)}
+    if cfg["feature_cache"] and cfg["engine"] in ("lookahead", "pairnet"):
+        batches.add(cfg["batch"])
+    return batches
 
 
 def batch_rows(B):
@@ -146,15 +198,19 @@ def _stack(clips, t, M):
             [np.stack([c["poses"][ms[m]] for c, (_, ms) in zip(clips, f)]) for m in range(M)], np.stack([c["K"] for c in clips]))
 
 
-def build_modules(n_depth_levels, device):
-    """bench.py's module set (seed-7 synthetic weights); aggregator0 reads D + 32 channels, so the modules are built under
-    Config.train_n_depth_levels = D as bench.py does for its c3 point"""
+def build_modules(n_depth_levels, device, pairnet=False):
+    """bench.py's module set, or pairnet's (dvmvs.pairnet.model: no LSTMFusion), with seed-7 synthetic weights; aggregator0 reads
+    D + 32 channels, so the modules are built under Config.train_n_depth_levels = D as bench.py does for its c3 point"""
     from dvmvs.config import Config
-    from dvmvs.fusionnet.model import CostVolumeDecoder, CostVolumeEncoder, FeatureExtractor, FeatureShrinker, LSTMFusion
+    from dvmvs.fusionnet import model as fusionnet
+    from dvmvs.pairnet import model as pairnet_model
+    mm = pairnet_model if pairnet else fusionnet
     saved = Config.train_n_depth_levels
     Config.train_n_depth_levels = n_depth_levels
     try:
-        mods = {"fe": FeatureExtractor(), "fpn": FeatureShrinker(), "cve": CostVolumeEncoder(), "lstm": LSTMFusion(), "cvd": CostVolumeDecoder()}
+        mods = {"fe": mm.FeatureExtractor(), "fpn": mm.FeatureShrinker(), "cve": mm.CostVolumeEncoder(), "cvd": mm.CostVolumeDecoder()}
+        if not pairnet:
+            mods["lstm"] = fusionnet.LSTMFusion()
     finally:
         Config.train_n_depth_levels = saved
     for m in mods.values():
@@ -165,9 +221,10 @@ def build_modules(n_depth_levels, device):
 
 
 def _drive(cfg, mods, dev, frames, rec_stream):
-    """runs the point's engine the way bench.py does before its timed region: prime() for the multi-stream engines (the
-    feature-cache engine primes with unique frame ids: every measurement frame misses and runs the eager feature pass), two
-    keyframes for the graphed engine and for the script's call sequence (the second one with recurrent state)"""
+    """runs the point's engine the way bench.py, tools/pairnet_bench.py and tools/lookahead_cache_bench.py do before their timed
+    regions: prime() for the multi-stream engines (the feature-cache engines prime with unique frame ids: every measurement frame
+    misses and runs the eager feature pass), two keyframes for the graphed engine and for the script's call sequence (the
+    second one with recurrent state).  Returns the engine (None for the script's call sequence)."""
     from dvmvs import pipeline
     kw = dict(batch=cfg["batch"], height=cfg["height"], width=cfg["width"], n_measurement_frames=cfg["n_measurement_frames"],
               n_depth_levels=cfg["n_depth_levels"])
@@ -177,36 +234,39 @@ def _drive(cfg, mods, dev, frames, rec_stream):
             for f in frames:
                 _, st = pipeline.keyframe(mods, st, *f, n_depth_levels=cfg["n_depth_levels"], batch_features=False)
             torch.cuda.synchronize(dev)
-            return
+            return None
         if cfg["engine"] == "graphed":
             eng = pipeline.GraphedFusionnet(mods, **kw)
             for f in frames:
                 eng.step(*f)
             torch.cuda.synchronize(dev)
-            return
-        if cfg["engine"] == "lookahead":
-            eng = pipeline.LookaheadFusionnet(mods, lookahead=cfg["lookahead"], **kw)
+            return eng
+        if cfg["engine"] in ("lookahead", "pairnet"):
+            cls = pipeline.LookaheadPairnet if cfg["engine"] == "pairnet" else pipeline.LookaheadFusionnet
+            eng = cls(mods, lookahead=cfg["lookahead"], feature_cache=cfg["feature_cache"], **kw)
         else:
             eng = pipeline.PipelinedFusionnet(mods, n_stages=cfg["n_stages"], feature_cache=cfg["feature_cache"], **kw)
         rec_stream.append(eng.streams[-1])
         eng.prime(*frames[0])
         eng.synchronize()
+        return eng
 
 
-def engine_calls(ops_recorded=("conv2d_tc",), height=None, width=None, device="cuda", native=None, point="value"):
-    """Builds one of bench.py's engines (POINTS[point]: seed-7 weights, tensor-core backend, the point's operand terms, batch,
-    input size, D and M; height / width override the input size), runs it as bench.py does before timing (_drive) with clip c
-    in batch row c, and records every call of the named functions of dvmvs._ops ("conv2d_tc", "conv2d_halo", "expand_dwconv",
-    "lstm_gates", "plane_sweep_tc", ...): returns (mods, {key: (args, kwargs, ConvLayer or None, on the recurrent stage?)}).
+def engine_calls(ops_recorded=("conv2d_tc",), height=None, width=None, device="cuda", native=None, point="value", engine=None):
+    """Builds the engine of an operating point (POINTS[point] or ENGINE_POINTS[point]: seed-7 weights, tensor-core backend, the
+    point's operand terms, batch, lookahead, feature cache, input size, D and M; height / width override the input size), runs
+    it as its benchmark does before timing (_drive) with clip c in batch row c, and records every call of the named functions of
+    dvmvs._ops ("conv2d_tc", "conv2d_halo", "expand_dwconv", "lstm_gates", "plane_sweep_tc", ...): returns
+    (mods, {key: (args, kwargs, ConvLayer or None, on the engine's last stream (last_stage)?)}).
     Each call site keeps its LAST call -- the one of the steady-state graph the engine replays, with recurrent state where
     the site has one -- on the engine's own buffers: their contents are whatever the engine left in them.
     native: a dict filled with {dvmvs_* entry point: number of calls} of every native call made meanwhile, and for dvmvs_conv2d
-    {"dvmvs_conv2d " + conv2d_branch: number of calls}."""
+    {"dvmvs_conv2d " + conv2d_branch: number of calls}.  engine: a list the driven engine is appended to."""
     cfg = point_config(point, height, width)
     ops.set_conv_backend("tc", terms=cfg["terms"], stride2=True)
     dev = torch.device(device, 0)
     H, W, M, B = cfg["height"], cfg["width"], cfg["n_measurement_frames"], cfg["batch"]
-    mods = build_modules(cfg["n_depth_levels"], dev)
+    mods = build_modules(cfg["n_depth_levels"], dev, pairnet=cfg["engine"] == "pairnet")
     clips = [synth.make_clip(c, 2, H, W, M) for c in range(B)]
     frames = []
     for t in range(2):
@@ -265,7 +325,9 @@ def engine_calls(ops_recorded=("conv2d_tc",), height=None, width=None, device="c
                 setattr(L, sym, native_recorder(sym))
     ops.ConvLayer.run, ops.ConvLayer.run_deferred = within(real_run), within(real_deferred)
     try:
-        _drive(cfg, mods, dev, frames, rec_stream)
+        eng = _drive(cfg, mods, dev, frames, rec_stream)
+        if engine is not None:
+            engine.append(eng)
     finally:
         for name, fn in real.items():
             setattr(ops, name, fn)
