@@ -12,6 +12,10 @@
 //                            (atomicCAS on the key, the pool slot from an atomic counter) and the block's slot appended to the
 //                            frame's list of visible blocks
 //   sparse_integrate_kernel  one thread per voxel of the listed blocks, a CTA half a block
+// Halt mode (include/dvmvs_tsdf_sparse_grow.h, counters[3]): sparse_box_kernel, the frame's first reader of the counters after
+// the previous frame's launches, decides once whether the frame starts with a pool- or table-full flag; if so its box is empty,
+// so sparse_alloc_kernel inserts nothing.  sparse_integrate_kernel reads the flags after the frame's own allocation, so the
+// frame that sets one is not integrated either.  sparse_rehash_kernel rebuilds the table of a grown pool.
 // Conservative test of a candidate block.  Its voxels' world points lie in the box spanned by its corner voxels' points (the
 // float32 rounding of origin + voxel_size * index is monotonic in the index), so their exact camera coordinates lie in the
 // parallelepiped of the 8 corners' camera coordinates.  Those are evaluated in float64 with a slack eps of 2^-40 times the
@@ -24,6 +28,7 @@
 #include <math.h>
 
 #include "../../include/dvmvs_tsdf_sparse.h"
+#include "../../include/dvmvs_tsdf_sparse_grow.h"
 #include "tsdf_block_hash.cuh"
 #include "tsdf_voxel.cuh"
 
@@ -32,6 +37,12 @@ namespace dvmvs {
 constexpr int kTile = 16;                            // pixels per tile edge of the max-depth image
 constexpr long long kMaxCandidates = 1ll << 31;
 constexpr int kBoxBytes = 64;                        // scratch head: SparseBox
+constexpr int kCapacityFlags = DVMVS_SPARSE_POOL_FULL | DVMVS_SPARSE_TABLE_FULL;
+
+// halt mode is on and a frame found no room: later frames (and the rest of this one's launches) leave the volume alone
+__device__ __forceinline__ bool sparse_halted(const int* counters) {
+  return (counters[3] & DVMVS_SPARSE_HALT_ON_FULL) && (counters[1] & kCapacityFlags);
+}
 
 struct SparseBox {
   int lo[3], n[3];
@@ -81,6 +92,25 @@ __device__ int sparse_insert(const SparseTable& t, int bx, int by, int bz) {
   return -1;
 }
 
+// one thread per pool slot of a grown pool: its key into the fresh table with its own slot.  The keys are distinct and the
+// table has >= 2 n_blocks entries, so every probe sequence reaches an empty entry.  Thread 0 resets the counters.
+__global__ void __launch_bounds__(256) sparse_rehash_kernel(unsigned long long* keys, int* slots, int mask, const int* __restrict__ coords,
+                                                            int n_blocks, int* counters) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int stride = gridDim.x * blockDim.x;
+  for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n_blocks; s += stride) {
+    const unsigned long long key = block_key(coords[3 * s], coords[3 * s + 1], coords[3 * s + 2]);
+    unsigned h = block_hash(key, mask);
+    while (atomicCAS(&keys[h], kEmpty, key) != kEmpty) h = (h + 1) & (unsigned)mask;
+    slots[h] = s;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    counters[0] = n_blocks;
+    counters[1] &= ~kCapacityFlags;
+  }
+}
+
 __device__ __forceinline__ double voxel_world(const SparseFrame& f, int axis, long long g) {
   return (double)__double2float_rn(__dadd_rn((double)f.origin[axis], __dmul_rn(f.voxel_size, (double)g)));
 }
@@ -107,7 +137,7 @@ __global__ void __launch_bounds__(256) sparse_tile_max_kernel(const DepthT* __re
   }
 }
 
-// one CTA: the frame's largest depth, then its candidate box; resets the frame's visible-block count
+// one CTA: the frame's largest depth, then its candidate box (empty when halted); resets the frame's visible-block count
 __global__ void __launch_bounds__(256) sparse_box_kernel(SparseFrame f, const double* __restrict__ tile_max, SparseBox* box,
                                                          int* counters) {
   pdl_launch_dependents();
@@ -123,7 +153,7 @@ __global__ void __launch_bounds__(256) sparse_box_kernel(SparseFrame f, const do
   for (int i = 1; i < 8; ++i) d = fmax(d, warp_max[i]);
   counters[2] = 0;
   SparseBox b = {{0, 0, 0}, {0, 0, 0}, 0};
-  if (d > 0.0) {
+  if (d > 0.0 && !sparse_halted(counters)) {
     const double zfar = (d + f.trunc) * (1.0 + 1e-9) + 1e-9;
     bool ok = isfinite(zfar);
     long long count = 1;
@@ -229,6 +259,7 @@ __global__ void __launch_bounds__(256) sparse_integrate_kernel(TsdfParams p, con
                                                                const int* __restrict__ visible, int capacity) {
   pdl_launch_dependents();
   pdl_wait();
+  if (sparse_halted(counters)) return;
   const int n_jobs = 2 * min(counters[2], capacity);
   const int lx = threadIdx.x >> 6, ly = (threadIdx.x >> 3) & 7, lz = threadIdx.x & 7;
   int hits = 0;
@@ -423,4 +454,17 @@ extern "C" int dvmvs_tsdf_sparse_block_bounds(const int* block_coords, int capac
   DVMVS_REQUIRE(capacity > 0, "tsdf_sparse_block_bounds: capacity %d", capacity);
   launch_k(sparse_bounds_kernel, dim3(1), dim3(1024), 0, (cudaStream_t)stream, block_coords, counters, capacity, bounds6);
   return check_launch("sparse_bounds_kernel");
+}
+
+extern "C" int dvmvs_tsdf_sparse_rehash(unsigned long long* keys, int* slots, int table_size, const int* block_coords, int n_blocks, int* counters,
+                                        dvmvs_stream_t stream) {
+  DVMVS_REQUIRE(keys && slots && block_coords && counters, "tsdf_sparse_rehash: null argument");
+  DVMVS_REQUIRE(table_size > 0 && table_size <= (1 << 30) && (table_size & (table_size - 1)) == 0 && n_blocks >= 0 &&
+                    2ll * n_blocks <= table_size,
+                "tsdf_sparse_rehash: table size %d, %d blocks (a power of two <= 2^30, >= 2 x the blocks)", table_size, n_blocks);
+  int grid = (n_blocks + 255) / 256;
+  grid = grid < 1 ? 1 : (grid > sparse_grid() ? sparse_grid() : grid);
+  launch_k(sparse_rehash_kernel, dim3(grid), dim3(256), 0, (cudaStream_t)stream, keys, slots, table_size - 1, block_coords, n_blocks,
+           counters);
+  return check_launch("sparse_rehash_kernel");
 }

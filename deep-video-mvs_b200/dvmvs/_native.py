@@ -37,6 +37,9 @@ SPARSE_POOL_FULL, SPARSE_TABLE_FULL, SPARSE_FRUSTUM = 1, 2, 4
 SPARSE_VIEW_SYMBOLS = [
     "dvmvs_tsdf_sparse_mesh_scratch_bytes", "dvmvs_tsdf_sparse_mesh_count", "dvmvs_tsdf_sparse_mesh_extract", "dvmvs_tsdf_sparse_raycast",
 ]
+# every symbol include/dvmvs_tsdf_sparse_grow.h declares (growing the voxel-block volume; tests/test_tsdf_sparse_grow.py covers them)
+SPARSE_GROW_SYMBOLS = ["dvmvs_tsdf_sparse_rehash"]
+SPARSE_HALT_ON_FULL = 1      # counters[3] bit of include/dvmvs_tsdf_sparse_grow.h
 
 
 class ConvDesc(ctypes.Structure):
@@ -156,6 +159,7 @@ def lib():
                                                   ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_double), d, p, p]
         L.dvmvs_tsdf_sparse_export.argtypes = [p, p, p, p, i, p, ctypes.POINTER(ctypes.c_int), i, i, i, p, p, p, p]
         L.dvmvs_tsdf_sparse_block_bounds.argtypes = [p, i, p, p, p]
+        L.dvmvs_tsdf_sparse_rehash.argtypes = [p, p, i, p, i, p, p]
         llp, fp3 = ctypes.POINTER(ll), ctypes.POINTER(ctypes.c_float)
         L.dvmvs_tsdf_sparse_mesh_scratch_bytes.argtypes = [i, llp]
         L.dvmvs_tsdf_sparse_mesh_count.argtypes = [p, p, i, p, i, p, p, i, llp, i, i, i, p, ll, p]

@@ -22,6 +22,7 @@ depth against ground truth with dvmvs.errors.compute_errors or as model-to-frame
 allocated on the device as frames see them (csrc/tsdf_sparse.cu) and hold what a TSDFVolume with the same origin holds after
 the same frames; `to_dense` exports any lattice-aligned box of it as a TSDFVolume, and its mesh and render methods return
 exactly what the export's would, computed on the blocks without the dense box (csrc/tsdf_sparse_view.cu)."""
+import collections
 import contextlib
 import ctypes
 
@@ -35,24 +36,31 @@ from ._ops import _stream
 class _FrameInputs(object):
     """Frame inputs of integrate on the volume's device: numpy arrays through pinned staging, CUDA tensors in place."""
 
-    def _upload(self, a, name):
+    def _upload(self, a, name, dst=None):
         """Host array -> device through a two-deep ring of pinned staging buffers owned by the volume (allocating pinned
-        memory per frame would cost more than the kernel); a slot is reused only after its previous copy has completed."""
+        memory per frame would cost more than the kernel); a slot is reused only after its previous copy has completed.
+        The copy lands in dst when given (a device tensor of a's shape and dtype), else in a device buffer of the slot."""
         key = (name, tuple(a.shape), a.dtype)
         ring = self._staging.get(key)
         if ring is None:
-            ring = self._staging[key] = {"next": 0, "slots": [
-                (torch.empty(a.shape, dtype=a.dtype).pin_memory(), torch.empty(a.shape, dtype=a.dtype, device=self.device), torch.cuda.Event())
-                for _ in range(2)]}
-        host, dev, done = ring["slots"][ring["next"]]
+            ring = self._staging[key] = {"next": 0, "slots": [[torch.empty(a.shape, dtype=a.dtype).pin_memory(), None, torch.cuda.Event()]
+                                                              for _ in range(2)]}
+        slot = ring["slots"][ring["next"]]
         ring["next"] ^= 1
+        host, done = slot[0], slot[2]
         done.synchronize()
         host.copy_(a)
-        dev.copy_(host, non_blocking=True)
+        if dst is None:
+            if slot[1] is None:
+                slot[1] = torch.empty(a.shape, dtype=a.dtype, device=self.device)
+            dst = slot[1]
+        dst.copy_(host, non_blocking=True)
         done.record()
-        return dev
+        return dst
 
-    def _to_device(self, a, allowed, name):
+    def _to_device(self, a, allowed, name, keep=None):
+        """a on the volume's device in an allowed dtype; keep(name, a) -> a device tensor of a's shape and dtype that the
+        result is copied into (a numpy array is uploaded straight into it), else a CUDA tensor is used in place"""
         if isinstance(a, np.ndarray):
             a = torch.from_numpy(np.ascontiguousarray(a))
         if not isinstance(a, torch.Tensor):
@@ -60,15 +68,17 @@ class _FrameInputs(object):
         if a.dtype not in allowed:
             a = a.to(allowed[-1])
         if not a.is_cuda:
-            return self._upload(a, name)
+            return self._upload(a, name, None if keep is None else keep(name, a))
         if a.device != self.device:
             raise RuntimeError("%s.integrate: %s lives on %s, the volume on %s" % (type(self).__name__, name, a.device, self.device))
-        return a.contiguous()
+        if keep is None:
+            return a.contiguous()
+        return keep(name, a).copy_(a)
 
-    def _frame(self, color_im, depth_im):
-        """(colour, depth) on the device, checked for shape"""
-        depth = self._to_device(depth_im, (torch.float64, torch.float32), "depth_im")
-        color = self._to_device(color_im, (torch.uint8, torch.float32), "color_im")
+    def _frame(self, color_im, depth_im, keep=None):
+        """(colour, depth) on the device, checked for shape (keep: as _to_device's)"""
+        depth = self._to_device(depth_im, (torch.float64, torch.float32), "depth_im", keep)
+        color = self._to_device(color_im, (torch.uint8, torch.float32), "color_im", keep)
         if depth.dim() != 2 or tuple(color.shape) != (depth.shape[0], depth.shape[1], 3):
             raise RuntimeError("%s.integrate: expected depth (H,W) and colour (H,W,3), got %s and %s" % (
                 type(self).__name__, tuple(depth.shape), tuple(color.shape)))
@@ -239,6 +249,13 @@ class TSDFVolume(_FrameInputs):
         return tuple(t.cpu().numpy() for t in self.render_tensors(cam_intr, cam_poses, height, width))
 
 
+_CAPACITY_FLAGS = N.SPARSE_POOL_FULL | N.SPARSE_TABLE_FULL
+# a frame a growable SparseTSDFVolume holds until its allocation is known to have found room: its ring slot (the device copies
+# of its depth and colour, the pinned copy of the counters after its allocation and the event recorded after that copy), its
+# number among the volume's integrate calls and integrate's arguments
+_HeldFrame = collections.namedtuple("_HeldFrame", "slot index color depth intr4 inv16 obs_weight")
+
+
 class SparseTSDFVolume(_FrameInputs):
     """TSDF fusion without bounds: a volume of 8 x 8 x 8-voxel blocks on the device (csrc/tsdf_sparse.cu, C ABI
     include/dvmvs_tsdf_sparse.h).  A frame allocates, through a hash table on the device, every block holding a voxel it can
@@ -250,10 +267,34 @@ class SparseTSDFVolume(_FrameInputs):
     on the blocks.
 
     Allocation runs on the device; integrate reads nothing back.  A pool of capacity_blocks blocks is allocated up front
-    (device_bytes tells its size).  When a frame needs more blocks than the pool holds, the blocks without room are not
-    integrated and the next allocated_blocks / to_dense raises RuntimeError naming the capacity the frames need; the blocks
-    that have room keep being integrated correctly."""
+    (device_bytes tells its size).  With max_capacity_blocks None (the default) the pool is fixed: when a frame needs more
+    blocks than it holds, the blocks without room are not integrated and the next allocated_blocks / to_dense / get_mesh* /
+    render* raises RuntimeError naming the capacity the frames need; the blocks that have room keep being integrated correctly.
+
+    With max_capacity_blocks an integer (>= capacity_blocks, at most 2^29) the volume grows, up to that many blocks, when its
+    frames need more.  A frame that finds the pool or the table full is not integrated, and neither is any later frame until
+    the volume has grown (halt mode, include/dvmvs_tsdf_sparse_grow.h).  integrate keeps each frame's depth and colour in a
+    ring of RING slots on the device until the host has seen, through a pinned copy of the counters, that its allocation found
+    room; it never synchronises, except that with all RING slots held it waits for the oldest frame's allocation.  When a held
+    frame turns out to have overflowed, and at the start of every read that synchronises (allocated_blocks, updated_voxels,
+    to_dense, get_mesh*, render*), the volume settles: it synchronises, grows the pool to
+    min(max_capacity_blocks, max(2 x capacity, blocks needed)) with the old pool's slots copied over and the hash table rebuilt
+    on the device (dvmvs_tsdf_sparse_rehash), replays the held frames from the first that overflowed, and repeats while a
+    frame still overflows.  **Contract**: after any frames, a growable volume holds, voxel for voxel, what a fixed volume
+    large enough from the start holds after the same frames, and so what a TSDFVolume with the same origin holds;
+    updated_voxels, to_dense, get_mesh* and render* return the same results too.  Only the order of the pool's slots differs
+    (it was never deterministic: slots come from an atomic counter, and none of those results depend on it).  At
+    max_capacity_blocks the frames from the one that overflowed on are not integrated (integrate then returns at once);
+    allocated_blocks, to_dense, get_mesh*
+    and render* then raise RuntimeError naming the blocks needed and the cap (updated_voxels still returns its count), and
+    every block with a slot holds what it held after the frames before that one.  `capacity` is the current pool size and
+    `growths` counts the growths so far."""
     BLOCK = 8
+    # Frames a growable volume holds on the device.  A frame is held until the copy of the counters behind its allocation has
+    # reached the host, a few launches after integrate enqueued it; 4 slots let the host run three frames ahead of the device
+    # (a depth network producing frames while the previous ones fuse) before integrate waits, at a cost of 4 frames of depth
+    # and colour in device memory (about 8.6 MB at 640 x 480 with float32 depth and uint8 colour).
+    RING = 4
 
     @staticmethod
     def table_size(capacity_blocks):
@@ -263,11 +304,18 @@ class SparseTSDFVolume(_FrameInputs):
     @staticmethod
     def device_bytes(capacity_blocks):
         """device memory of a volume with capacity_blocks blocks: 512 voxels x 12 B, block coordinates and the visible list
-        per block; 8 B key and 4 B slot per hash-table entry; the counters"""
+        per block; 8 B key and 4 B slot per hash-table entry; the counters.  A growable volume (max_capacity_blocks) holds
+        both pools for the length of a growth: its device memory peaks at device_bytes(old capacity) + device_bytes(new
+        capacity), plus its ring of RING frames."""
         c = int(capacity_blocks)
         return c * (SparseTSDFVolume.BLOCK ** 3 * 12 + 12 + 4) + SparseTSDFVolume.table_size(c) * 12 + 16
 
-    def __init__(self, voxel_size, origin=(0.0, 0.0, 0.0), capacity_blocks=32768, device=None):
+    @staticmethod
+    def _grown_capacity(capacity, need, max_capacity):
+        """the pool a growth allocates: at least double the current one and at least the blocks needed, at most the cap"""
+        return min(int(max_capacity), max(2 * int(capacity), int(need)))
+
+    def __init__(self, voxel_size, origin=(0.0, 0.0, 0.0), capacity_blocks=32768, device=None, max_capacity_blocks=None):
         voxel_size = float(voxel_size)
         if not (np.isfinite(voxel_size) and voxel_size > 0):
             raise ValueError("SparseTSDFVolume: voxel_size must be finite and > 0, got %r" % voxel_size)
@@ -279,6 +327,14 @@ class SparseTSDFVolume(_FrameInputs):
         capacity = int(capacity_blocks)
         if self.table_size(capacity) > 1 << 30:
             raise ValueError("SparseTSDFVolume: capacity_blocks %d exceeds 2^29" % capacity)
+        if max_capacity_blocks is not None:
+            if (isinstance(max_capacity_blocks, bool) or int(max_capacity_blocks) != max_capacity_blocks
+                    or max_capacity_blocks < capacity):
+                raise ValueError("SparseTSDFVolume: max_capacity_blocks must be None or an integer >= capacity_blocks %d, got %r"
+                                 % (capacity, max_capacity_blocks))
+            max_capacity_blocks = int(max_capacity_blocks)
+            if self.table_size(max_capacity_blocks) > 1 << 30:
+                raise ValueError("SparseTSDFVolume: max_capacity_blocks %d exceeds 2^29" % max_capacity_blocks)
         if not N.DRYRUN and not torch.cuda.is_available():
             raise RuntimeError("SparseTSDFVolume: needs a CUDA device (no CPU fallback)")
         self._voxel_size = voxel_size
@@ -297,11 +353,20 @@ class SparseTSDFVolume(_FrameInputs):
         self._tsdf = torch.ones((capacity, b, b, b), dtype=torch.float32, device=dev)   # TSDFVolume's initial state (:57-61)
         self._weight = torch.zeros((capacity, b, b, b), dtype=torch.float32, device=dev)
         self._color = torch.zeros((capacity, b, b, b), dtype=torch.float32, device=dev)
-        self._counters = torch.zeros(4, dtype=torch.int32, device=dev)                 # keys, flags, visible, unused
+        self._counters = torch.zeros(4, dtype=torch.int32, device=dev)                 # keys, flags, visible, halt mode
         self._visible = torch.zeros(capacity, dtype=torch.int32, device=dev)
         self._updated = torch.zeros(1, dtype=torch.int64, device=dev)
         self._scratch = {}
         self._staging = {}
+        self.max_capacity_blocks = max_capacity_blocks
+        self.growths = 0
+        self._held = collections.deque()                 # growable: the frames not yet known to have found room, oldest first
+        self._ring = [{} for _ in range(self.RING)]      # per ring slot: name -> device copy of that input
+        self._ring_flags = self._ring_events = None      # pinned [RING][2] counters[0:2] after each slot's allocation; events
+        self._next_slot = self._frames = 0
+        self._halted_at = None                           # at max_capacity_blocks: the first frame not integrated
+        if max_capacity_blocks is not None:
+            self._counters[3] = N.SPARSE_HALT_ON_FULL
 
     def _device_scope(self):
         return torch.cuda.device(self.device) if self.device.type == "cuda" else contextlib.nullcontext()
@@ -309,35 +374,136 @@ class SparseTSDFVolume(_FrameInputs):
     # ---- the hot path -------------------------------------------------------------------------------------------------
     def integrate(self, color_im, depth_im, cam_intr, cam_pose, obs_weight=1.):
         """Integrate an RGB-D frame: TSDFVolume.integrate's arguments, accepted types and arithmetic (:220-323), with the
-        blocks the frame can update allocated first.  Focal lengths must be finite and > 0."""
+        blocks the frame can update allocated first.  Focal lengths must be finite and > 0.  A growable volume copies the
+        frame's depth and colour to its ring first: the caller may overwrite its tensors as soon as integrate returns."""
         intr4, inv16 = self._camera(cam_intr, cam_pose)
         if not (np.all(np.isfinite(list(intr4))) and intr4[0] > 0 and intr4[1] > 0):
             raise ValueError("SparseTSDFVolume.integrate: focal lengths must be finite and > 0 and the principal point finite, "
                              "got fx %r fy %r cx %r cy %r" % tuple(intr4))
         with self._device_scope():
-            color, depth = self._frame(color_im, depth_im)
-            h, w = int(depth.shape[0]), int(depth.shape[1])
-            scratch = self._scratch.get((h, w))
-            if scratch is None:
-                nbytes = ctypes.c_longlong(0)
-                N.check(N.lib().dvmvs_tsdf_sparse_scratch_bytes(h, w, ctypes.byref(nbytes)), "tsdf_sparse_scratch_bytes")
-                scratch = self._scratch[(h, w)] = torch.empty(max(int(nbytes.value), 8), dtype=torch.uint8, device=self.device)
-            depth_f64 = 1 if depth.dtype == torch.float64 else 0
-            stream = _stream()
-            N.check(N.lib().dvmvs_tsdf_sparse_allocate(
-                self._keys.data_ptr(), self._slots.data_ptr(), int(self._keys.numel()), self._coords.data_ptr(), self.capacity,
-                self._counters.data_ptr(), self._visible.data_ptr(), scratch.data_ptr(), scratch.numel(), self._origin_c,
-                self._voxel_size, self._trunc_margin, depth.data_ptr(), depth_f64, h, w, intr4, inv16, stream), "tsdf_sparse_allocate")
-            N.check(N.lib().dvmvs_tsdf_sparse_integrate(
-                self._tsdf.data_ptr(), self._weight.data_ptr(), self._color.data_ptr(), self._coords.data_ptr(), self.capacity,
-                self._counters.data_ptr(), self._visible.data_ptr(), self._origin_c, self._voxel_size, self._trunc_margin,
-                color.data_ptr(), 1 if color.dtype == torch.uint8 else 0, depth.data_ptr(), depth_f64, h, w, intr4, inv16,
-                float(obs_weight), self._updated.data_ptr(), stream), "tsdf_sparse_integrate")
+            if self.max_capacity_blocks is None:
+                color, depth = self._frame(color_im, depth_im)
+                self._enqueue(color, depth, intr4, inv16, float(obs_weight))
+                return
+            if self._halted_at is not None:
+                return                                                      # at the cap: no later frame is integrated
+            if self._ring_events is None:
+                self._ring_flags = torch.zeros((self.RING, 2), dtype=torch.int32).pin_memory()
+                self._ring_events = [torch.cuda.Event() for _ in range(self.RING)]
+            self._retire()
+            if len(self._held) == self.RING:
+                self._ring_events[self._held[0].slot].synchronize()        # integrate's one wait: RING frames in flight
+                self._retire()
+            slot = self._next_slot
+            color, depth = self._frame(color_im, depth_im, keep=lambda name, a: self._ring_buffer(slot, name, a))
+            frame = _HeldFrame(slot, self._frames, color, depth, intr4, inv16, float(obs_weight))
+            # held only once the library has accepted the frame: a frame it refuses (a pose that is not an invertible finite
+            # transform) raises here, before any launch, and takes no ring slot, so no replay ever meets it
+            self._enqueue(color, depth, intr4, inv16, frame.obs_weight, slot)
+            self._next_slot, self._frames = (slot + 1) % self.RING, self._frames + 1
+            self._held.append(frame)
+
+    def _enqueue(self, color, depth, intr4, inv16, obs_weight, slot=None):
+        """allocate + integrate one frame on the current stream, inside the volume's device scope; with a ring slot, the
+        counters after the allocation are copied to the slot's pinned entry and its event recorded"""
+        h, w = int(depth.shape[0]), int(depth.shape[1])
+        scratch = self._scratch.get((h, w))
+        if scratch is None:
+            nbytes = ctypes.c_longlong(0)
+            N.check(N.lib().dvmvs_tsdf_sparse_scratch_bytes(h, w, ctypes.byref(nbytes)), "tsdf_sparse_scratch_bytes")
+            scratch = self._scratch[(h, w)] = torch.empty(max(int(nbytes.value), 8), dtype=torch.uint8, device=self.device)
+        depth_f64 = 1 if depth.dtype == torch.float64 else 0
+        stream = _stream()
+        N.check(N.lib().dvmvs_tsdf_sparse_allocate(
+            self._keys.data_ptr(), self._slots.data_ptr(), int(self._keys.numel()), self._coords.data_ptr(), self.capacity,
+            self._counters.data_ptr(), self._visible.data_ptr(), scratch.data_ptr(), scratch.numel(), self._origin_c,
+            self._voxel_size, self._trunc_margin, depth.data_ptr(), depth_f64, h, w, intr4, inv16, stream), "tsdf_sparse_allocate")
+        if slot is not None:
+            self._ring_flags[slot].copy_(self._counters[:2], non_blocking=True)
+            self._ring_events[slot].record()
+        N.check(N.lib().dvmvs_tsdf_sparse_integrate(
+            self._tsdf.data_ptr(), self._weight.data_ptr(), self._color.data_ptr(), self._coords.data_ptr(), self.capacity,
+            self._counters.data_ptr(), self._visible.data_ptr(), self._origin_c, self._voxel_size, self._trunc_margin,
+            color.data_ptr(), 1 if color.dtype == torch.uint8 else 0, depth.data_ptr(), depth_f64, h, w, intr4, inv16,
+            float(obs_weight), self._updated.data_ptr(), stream), "tsdf_sparse_integrate")
+
+    # ---- growth ---------------------------------------------------------------------------------------------------------
+    def _ring_buffer(self, slot, name, a):
+        """the ring slot's device buffer for input `name`, of a's shape and dtype"""
+        t = self._ring[slot].get(name)
+        if t is None or t.shape != a.shape or t.dtype != a.dtype:
+            t = self._ring[slot][name] = torch.empty(a.shape, dtype=a.dtype, device=self.device)
+        return t
+
+    def _overflowed(self, frame):
+        return bool(int(self._ring_flags[frame.slot, 1]) & _CAPACITY_FLAGS)
+
+    def _retire(self):
+        """lets go of the held frames whose allocation has completed, oldest first; one that found no room settles the volume
+        (which replays it and every later frame, and lets go of them all)"""
+        while self._held and self._ring_events[self._held[0].slot].query():
+            if self._halted_at is None and self._overflowed(self._held[0]):
+                self._settle()
+            else:
+                self._held.popleft()
+
+    def _synchronize(self):
+        if self.device.type == "cuda":
+            torch.cuda.synchronize(self.device)
+
+    def _settle(self):
+        """Synchronises; then, while a frame has found no room and max_capacity_blocks allows, grows the volume and replays
+        the held frames from the first that found none.  At the cap, records that frame.  Either way every held frame is then
+        settled -- integrated after the last growth, or never to be -- and is let go."""
+        if self.max_capacity_blocks is None or self._halted_at is not None:
+            return
+        with self._device_scope():
+            self._synchronize()
+            while True:
+                n, flags = (int(v) for v in self._counters[:2].tolist())
+                held = list(self._held)
+                if not flags & _CAPACITY_FLAGS:
+                    self._held.clear()
+                    return
+                first = next((i for i, f in enumerate(held) if self._overflowed(f)), 0)
+                if self.capacity >= self.max_capacity_blocks:
+                    self._halted_at = held[first].index if held else self._frames
+                    self._held.clear()
+                    return
+                self._grow(self._grown_capacity(self.capacity, n, self.max_capacity_blocks), min(n, self.capacity))
+                for f in held[first:]:
+                    self._enqueue(f.color, f.depth, f.intr4, f.inv16, f.obs_weight, f.slot)
+                self._synchronize()
+
+    def _grow(self, capacity, n_blocks):
+        """a pool of `capacity` blocks whose first slots are the old pool's, and a hash table of table_size(capacity) entries
+        rebuilt on the device from its first n_blocks slots; clears the pool- and table-full flags"""
+        dev, b, old = self.device, self.BLOCK, self.capacity
+        table = self.table_size(capacity)
+        grown = (torch.zeros((capacity, 3), dtype=torch.int32, device=dev), torch.ones((capacity, b, b, b), dtype=torch.float32, device=dev),
+                 torch.zeros((capacity, b, b, b), dtype=torch.float32, device=dev), torch.zeros((capacity, b, b, b), dtype=torch.float32, device=dev))
+        for new, cur in zip(grown, (self._coords, self._tsdf, self._weight, self._color)):
+            new[:old].copy_(cur)
+        self._coords, self._tsdf, self._weight, self._color = grown
+        self._visible = torch.zeros(capacity, dtype=torch.int32, device=dev)
+        self._keys = torch.full((table,), -1, dtype=torch.int64, device=dev)
+        self._slots = torch.full((table,), -1, dtype=torch.int32, device=dev)
+        N.check(N.lib().dvmvs_tsdf_sparse_rehash(self._keys.data_ptr(), self._slots.data_ptr(), table, self._coords.data_ptr(), n_blocks,
+                                                  self._counters.data_ptr(), _stream()), "tsdf_sparse_rehash")
+        self.capacity = capacity
+        self.growths += 1
 
     # ---- read-back ----------------------------------------------------------------------------------------------------
     def allocated_blocks(self):
-        """Number of blocks allocated so far (synchronises).  RuntimeError when a frame found no room for a block."""
+        """Number of blocks allocated so far (synchronises; a growable volume settles first).  RuntimeError when a frame
+        found no room for a block (a growable volume: at max_capacity_blocks)."""
+        self._settle()
         n, flags = (int(v) for v in self._counters[:2].cpu())
+        if self._halted_at is not None and flags & _CAPACITY_FLAGS:
+            raise RuntimeError("SparseTSDFVolume: the frames so far need %s blocks, more than max_capacity_blocks %d: frame %d "
+                               "(counting the frames integrate accepted from 0), the one that overflowed the volume, and every later frame "
+                               "were not integrated" % (("more than %d" if flags & N.SPARSE_TABLE_FULL else "%d") % n,
+                                                        self.max_capacity_blocks, self._halted_at))
         if flags & N.SPARSE_TABLE_FULL:
             raise RuntimeError("SparseTSDFVolume: the hash table of %d entries is full; the frames so far need more than %d "
                                "blocks: construct the volume with a larger capacity_blocks" % (self._keys.numel(), n))
@@ -350,7 +516,8 @@ class SparseTSDFVolume(_FrameInputs):
         return n
 
     def updated_voxels(self):
-        """Total number of voxel updates so far (synchronises)."""
+        """Total number of voxel updates so far (synchronises; a growable volume settles first)."""
+        self._settle()
         return int(self._updated.item())
 
     def _box(self, vol_bnds, what):

@@ -15,9 +15,10 @@
  *   block_coords[capacity][3] int32 block coordinates of each pool slot (block = floor(global voxel index / 8)) [any]
  *   tsdf, weight, color [capacity][8][8][8] fp32 voxels of each pool slot, x-major as the dense volume [1 / 0 / 0]
  *   counters    [4] int32: keys inserted (= pool slots the frames so far need), error flags (DVMVS_SPARSE_*), blocks the last
- *               allocated frame sees, unused [0 0 0 0]
+ *               allocated frame sees, halt mode (include/dvmvs_tsdf_sparse_grow.h; 0 = off) [0 0 0 0]
  *   visible     [capacity] int32 pool slots the last allocated frame sees (its first counters[2] entries) [any]
- * A flag never clears; a block the pool or the table had no room for is not integrated, and the flag says so.
+ * A flag never clears (only dvmvs_tsdf_sparse_rehash of include/dvmvs_tsdf_sparse_grow.h clears the pool- and table-full flags
+ * of a grown volume); a block the pool or the table had no room for is not integrated, and the flag says so.
  */
 #ifndef DVMVS_TSDF_SPARSE_H
 #define DVMVS_TSDF_SPARSE_H
