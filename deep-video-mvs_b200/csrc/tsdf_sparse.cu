@@ -7,7 +7,9 @@
 // Per frame, four launches and no host read:
 //   sparse_tile_max_kernel   largest valid depth (> 0; NaN never counts) of every 16 x 16-pixel tile
 //   sparse_box_kernel        the frame's largest depth D and the world box of its view frustum up to D + trunc: the candidate
-//                            blocks (blocks of that box, two voxels of margin)
+//                            blocks (blocks of that box; margin: one float32 spacing at the box's largest coordinate, which
+//                            bounds how far a voxel's rounded world point strays from origin + voxel_size * index, plus two
+//                            voxels)
 //   sparse_alloc_kernel      one thread per candidate block: a conservative test (below), then insertion into the hash table
 //                            (atomicCAS on the key, the pool slot from an atomic counter) and the block's slot appended to the
 //                            frame's list of visible blocks
@@ -164,8 +166,14 @@ __global__ void __launch_bounds__(256) sparse_box_kernel(SparseFrame f, const do
         lo = fmin(lo, p);
         hi = fmax(hi, p);
       }
-      // two voxels of margin, in voxel units relative to the origin, then blocks
-      const double vlo = floor((lo - (double)f.origin[a]) / f.voxel_size) - 2.0, vhi = floor((hi - (double)f.origin[a]) / f.voxel_size) + 2.0;
+      // A voxel the frame updates has its world point voxel_world(g) in [lo, hi], but the float32 rounding moves that point up
+      // to half a float32 spacing away from origin + voxel_size * g -- many voxels far from the origin (0.5 m at 4.2e6 m).  So
+      // the index range is widened by one float32 spacing at the box's largest magnitude, then by two voxels for the float64
+      // evaluation of the frustum and of these quotients, then taken to blocks.
+      const double m = fmax(fabs(lo), fabs(hi)) + 2.0 * f.voxel_size;
+      const double spacing = ldexp(1.0, ilogb(m) - 23);
+      const double vlo = floor((lo - spacing - (double)f.origin[a]) / f.voxel_size) - 2.0,
+                   vhi = floor((hi + spacing - (double)f.origin[a]) / f.voxel_size) + 2.0;
       const double blo = floor(vlo / kBlock), bhi = floor(vhi / kBlock);
       if (!(blo >= -(double)kKeyBias && bhi < (double)kKeyBias)) {
         ok = false;

@@ -6,6 +6,7 @@ frames.  A voxel the allocation missed would export weight 0 where the dense vol
 
 CPU: the header against the library and the ctypes binding, and (DVMVS_DRYRUN=1, in a subprocess) the constructor's argument
 checks, the capacity arithmetic, the lattice check of to_dense and the overflow messages."""
+import importlib
 import os
 import re
 import subprocess
@@ -21,9 +22,9 @@ import tsdf_cases  # noqa: E402
 
 from tests.test_tsdf import _rot, _same  # noqa: E402
 
-# every entry point of include/dvmvs_tsdf_sparse.h -> the test of this module that checks what it computes
+# every entry point of include/dvmvs_tsdf_sparse.h -> the test (of this module, or "module::test") that checks what it computes
 SPARSE_TESTS = {
-    "dvmvs_tsdf_sparse_allocate": "test_gpu_sparse_equals_dense_on_the_reference_cases",
+    "dvmvs_tsdf_sparse_allocate": "tests.test_tsdf_block_reference::test_gpu_allocation_frame_by_frame",
     "dvmvs_tsdf_sparse_integrate": "test_gpu_sparse_equals_dense_on_the_reference_cases",
     "dvmvs_tsdf_sparse_export": "test_gpu_unbounded_path_every_sub_box_equals_a_dense_volume_over_it",
     "dvmvs_tsdf_sparse_block_bounds": "test_gpu_unbounded_path_every_sub_box_equals_a_dense_volume_over_it",
@@ -37,6 +38,13 @@ def _header_prototypes():
     return re.findall(r"\bint\s+(dvmvs_[a-z0-9_]+)\s*\(([^)]*)\)\s*;", header)
 
 
+def _names_a_test(t):
+    if "::" in t:
+        mod, fn = t.split("::")
+        return callable(getattr(importlib.import_module(mod), fn, None))
+    return callable(globals().get(t))
+
+
 def test_sparse_header_library_binding_and_coverage_agree():
     """Every prototype of include/dvmvs_tsdf_sparse.h is exported, listed in SPARSE_SYMBOLS, bound with as many arguments of
     the same C classes, mapped to a test here (or host-only), and absent from dvmvs_b200.h's list."""
@@ -47,7 +55,7 @@ def test_sparse_header_library_binding_and_coverage_agree():
     assert names == sorted(N.SPARSE_SYMBOLS) and len(names) == 5
     assert not set(names) & set(N.EXPORTED_SYMBOLS)
     assert sorted(set(SPARSE_TESTS) | SPARSE_HOST_ONLY) == names and not set(SPARSE_TESTS) & SPARSE_HOST_ONLY
-    assert all(callable(globals().get(t)) for t in SPARSE_TESTS.values())
+    assert all(_names_a_test(t) for t in SPARSE_TESTS.values())
     lib = N.lib()
     kinds = {"ptr": (ctypes.c_void_p,), "int": (ctypes.c_int,), "longlong": (ctypes.c_longlong,), "double": (ctypes.c_double,)}
     for name, params in protos:
