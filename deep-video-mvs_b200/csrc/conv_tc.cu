@@ -356,6 +356,189 @@ __global__ void conv_tc_finish_kernel(TcParams p) {
   }
 }
 
+// ----------------------------------------------------------------------------------------------- weight-streaming split-K
+// Small-map 3x3 / 5x5 layers with many output channels (the ConvLSTM gate GEMM, the decoder's 16^2 / 32^2 blocks) are bound by
+// their weight stream, not by their MMAs.  conv_ws_kernel swaps the GEMM's operands so that the weights fill the MMA's M side:
+//
+//   D[128 output channels x NPIX output pixels] (fp32, registers) += W[128 x K] . A[NPIX x K]^T
+//
+// * A operand = 128 packed weight rows ([rows][K], K-major: the TMA box of conv_tc_kernel's weight map, 128 rows tall),
+//   two m64 blocks per warpgroup.  B operand = the tap-shifted activation box of make_act_map (zero fill = padding), NPIX =
+//   its pixels: an 8x8 box on maps of at most 8x8 (no padded half on the gate's 8x8 map), the 16x8 / 8x16 box elsewhere.
+// * Always split-K over the taps (ksplit >= 2); partial sums go to the workspace in conv_tc_kernel's layout
+//   [ksplit][B*Hout*Wout][Cout], so conv_tc_finish_kernel and dvmvs_lstm_gates_parts consume them unchanged.  The epilogue
+//   transposes the [channel][pixel] accumulators through shared memory: stores stay channel-contiguous.
+// * Operand terms in conv_tc_kernel's order: hi*hi (+ lo*hi + hi*lo), activation lo in the second, weight lo in the third.
+constexpr int kWsRows = 128;
+// split-count target (see tc_plan).  H100 80GB HBM3 at 700 W, bench.py's engine, targets alternated in one session:
+// 32 / 64 / 128 CTAs gave 2 078 / 2 122 / 2 100 keyframes/s (base 2 029)
+constexpr int kWsTargetCtas = 64;
+constexpr int kWsMaxPixels = 32 * 32;                 // output pixels per image up to which conv_ws_kernel is chosen
+constexpr int kWsRingBytes = 128 * 1024;
+constexpr long long kWsCounterBytes = 16384;          // reserved head of the split-K workspace (historical: arrival counters)
+
+template <int NPIX, int KSTEPS, int TERMS>
+__device__ __forceinline__ void ws_mma_chunk(float (&acc)[2][NPIX / 2], uint32_t sb, uint32_t off_w_lo, uint32_t off_a_hi,
+                                             uint32_t off_a_lo) {
+  constexpr uint32_t layout = (KSTEPS == 4) ? kGmmaSw128 : kGmmaSw64;
+  constexpr uint32_t sbo = KSTEPS * 256u;                 // 8 rows x row bytes
+  constexpr uint32_t half_rows = 64u * KSTEPS * 32u;      // byte offset of weight rows [64, 128)
+  wgmma_fence_regs(acc[0]);
+  wgmma_fence_regs(acc[1]);
+  wgmma_fence();
+#pragma unroll
+  for (int term = 0; term < TERMS; ++term) {
+    const uint32_t w_s = sb + ((term == 2) ? off_w_lo : 0u);
+    const uint32_t a_s = sb + ((term == 1) ? off_a_lo : off_a_hi);
+#pragma unroll
+    for (int k = 0; k < KSTEPS; ++k) {
+      const uint64_t bd = gmma_desc(a_s + 32u * k, 16u, sbo, layout);
+      wgmma_f16<NPIX>(acc[0], gmma_desc(w_s + 32u * k, 16u, sbo, layout), bd);
+      wgmma_f16<NPIX>(acc[1], gmma_desc(w_s + half_rows + 32u * k, 16u, sbo, layout), bd);
+    }
+  }
+  wgmma_commit();
+}
+
+template <int NPIX>
+__global__ void __launch_bounds__(kTcThreads) conv_ws_kernel(const __grid_constant__ TcParams p) {
+  pdl_launch_dependents();
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw_addr = smem_u32(smem_raw);
+  const uint32_t base = (raw_addr + 1023u) & ~1023u;
+  uint8_t* base_ptr = smem_raw + (base - raw_addr);
+  const int n_stages = p.num_stages;
+  const uint32_t bars = base + p.ring_bytes;
+  auto full_bar = [&](int s) { return bars + 8u * s; };
+  auto empty_bar = [&](int s) { return bars + 8u * (kMaxStages + s); };
+  // stage layout: weights hi [, weights lo], activations hi [, activations lo]
+  const uint32_t off_w_lo = p.w_bytes, off_a_hi = (p.terms > 1 ? 2u : 1u) * p.w_bytes, off_a_lo = off_a_hi + p.a_bytes;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tiles_per_img = p.tiles_x * p.tiles_y;
+  const int b = blockIdx.x / tiles_per_img;
+  const int t_in = blockIdx.x - b * tiles_per_img;
+  const int oy0 = (t_in / p.tiles_x) * p.tile_h, ox0 = (t_in % p.tiles_x) * p.tile_w;
+  const int m0 = blockIdx.y * kWsRows;
+  const int n_taps = p.ksize * p.ksize;
+  const int taps_per_split = (n_taps + p.ksplit - 1) / p.ksplit;
+  const int tap_begin = blockIdx.z * taps_per_split, tap_end = min(n_taps, tap_begin + taps_per_split);
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < p.n_src; ++s) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&p.a_map[s][0]) : "memory");
+      if (p.terms > 1) asm volatile("prefetch.tensormap [%0];" ::"l"(&p.a_map[s][1]) : "memory");
+    }
+    for (int s = 0; s < n_stages; ++s) {
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), 4);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (warp == 4) {
+    // ============================== TMA producer ==============================
+    if (lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tap = tap_begin; tap < tap_end; ++tap) {
+        const int ky = tap / p.ksize, kx = tap - ky * p.ksize;
+        const int iy = oy0 * p.stride - p.pad + ky, ix = ox0 * p.stride - p.pad + kx;
+        int wk = tap * p.k_per_tap;
+        for (int s = 0; s < p.n_src; ++s) {
+          const int kc = p.src_kchunk[s];
+          const int kind = (kc == 64) ? 1 : 0;
+          for (int ch = 0; ch < p.src_chunks[s]; ++ch, wk += kc) {
+            mbar_wait(empty_bar(stage), phase ^ 1u);
+            const uint32_t sb = base + stage * p.stage_bytes;
+            const uint32_t w_bytes = kWsRows * kc * 2, a_bytes = NPIX * kc * 2;
+            mbar_expect_tx(full_bar(stage), (p.terms > 1 ? 2u : 1u) * (a_bytes + w_bytes));
+            tma_load_2d(sb, &p.w_map[kind][0], full_bar(stage), wk, m0);
+            tma_load_4d(sb + off_a_hi, &p.a_map[s][0], full_bar(stage), ch * kc, ix, iy, b);
+            if (p.terms > 1) {
+              tma_load_2d(sb + off_w_lo, &p.w_map[kind][1], full_bar(stage), wk, m0);
+              tma_load_4d(sb + off_a_lo, &p.a_map[s][1], full_bar(stage), ch * kc, ix, iy, b);
+            }
+            if (++stage == n_stages) { stage = 0; phase ^= 1u; }
+          }
+        }
+      }
+    }
+  } else {
+    // ============================== MMA warpgroup (warps 0-3) ==============================
+    float acc[2][NPIX / 2];            // output channels [m0, m0 + 64) and [m0 + 64, m0 + 128)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < NPIX / 2; ++i) acc[h][i] = 0.f;
+    {
+      int stage = 0, prev_stage = -1;
+      uint32_t phase = 0;
+      for (int tap = tap_begin; tap < tap_end; ++tap) {
+        for (int s = 0; s < p.n_src; ++s) {
+          const int kc = p.src_kchunk[s];
+          for (int ch = 0; ch < p.src_chunks[s]; ++ch) {
+            mbar_wait(full_bar(stage), phase);
+            const uint32_t sb = base + stage * p.stage_bytes;
+            if (kc == 64) {
+              if (p.terms == 3) ws_mma_chunk<NPIX, 4, 3>(acc, sb, off_w_lo, off_a_hi, off_a_lo);
+              else ws_mma_chunk<NPIX, 4, 1>(acc, sb, off_w_lo, off_a_hi, off_a_lo);
+            } else {
+              if (p.terms == 3) ws_mma_chunk<NPIX, 2, 3>(acc, sb, off_w_lo, off_a_hi, off_a_lo);
+              else ws_mma_chunk<NPIX, 2, 1>(acc, sb, off_w_lo, off_a_hi, off_a_lo);
+            }
+            wgmma_wait<1>();
+            wgmma_fence_regs(acc[0]);
+            wgmma_fence_regs(acc[1]);
+            if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar(prev_stage));
+            prev_stage = stage;
+            if (++stage == n_stages) { stage = 0; phase ^= 1u; }
+          }
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc[0]);
+      wgmma_fence_regs(acc[1]);
+    }
+    // ============================== epilogue: partial sums -> workspace ==============================
+    // the ring becomes the fp32 staging tile [NPIX pixels][128 + 4 channels]: accumulator element 4j+e of thread (warp, lane)
+    // is channel 16 warp + lane/4 + 8 (e/2) of its m64 block, pixel 8j + 2 (lane%4) + e%2.  The pitch of 132 floats puts the
+    // four pixel columns of a warp's store 8 banks apart: conflict-free.
+    constexpr int kPitch = kWsRows + 4;
+    float* stg = reinterpret_cast<float*>(base_ptr);
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int c = h * 64 + warp * 16 + (lane >> 2);
+#pragma unroll
+      for (int j = 0; j < NPIX / 8; ++j) {
+        const int px = 8 * j + 2 * (lane & 3);
+        stg[px * kPitch + c] = acc[h][4 * j];
+        stg[(px + 1) * kPitch + c] = acc[h][4 * j + 1];
+        stg[px * kPitch + c + 8] = acc[h][4 * j + 2];
+        stg[(px + 1) * kPitch + c + 8] = acc[h][4 * j + 3];
+      }
+    }
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    const size_t plane_stride = (size_t)p.B * p.Hout * p.Wout * p.Cout;
+    float* wsp = p.workspace + (size_t)blockIdx.z * plane_stride;
+    constexpr int kChunks = kWsRows / 8;
+#pragma unroll 1
+    for (int item = threadIdx.x; item < NPIX * kChunks; item += 128) {
+      const int px = item / kChunks, c0 = 8 * (item - px * kChunks);
+      const int ty = px / p.tile_w, tx = px - ty * p.tile_w;
+      const int oy = oy0 + ty, ox = ox0 + tx;
+      const int cbase = m0 + c0;
+      if (oy >= p.Hout || ox >= p.Wout || cbase >= p.Cout) continue;     // Cout % 8 == 0: a chunk is all in or all out
+      float* o = wsp + (((size_t)b * p.Hout + oy) * p.Wout + ox) * p.Cout + cbase;
+      *reinterpret_cast<float4*>(o) = *reinterpret_cast<const float4*>(stg + px * kPitch + c0);
+      *reinterpret_cast<float4*>(o + 4) = *reinterpret_cast<const float4*>(stg + px * kPitch + c0 + 4);
+    }
+  }
+}
+
 // fp32 channel-last -> fp16 (hi, lo) planes with the channel count padded to Cs (zeros); optional x2 bilinear
 // (align_corners) upsampling on the way (materialises F.interpolate for the TMA-fed consumer).
 __global__ void split_planes_kernel(const float* __restrict__ x, __half* __restrict__ planes, int B, int H, int W, int C, int Cs,
@@ -568,6 +751,82 @@ static int launch_tc(TcParams& p, dim3 grid, int kc_max, cudaStream_t s) {
   return check_launch("conv_tc_kernel");
 }
 
+template <int NPIX>
+static int launch_ws(TcParams& p, dim3 grid, int kc_max, cudaStream_t s) {
+  static PerDeviceOnce attr_set;
+  if (attr_set.first()) {
+    cudaError_t e = cudaFuncSetAttribute(conv_ws_kernel<NPIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemBytes);
+    if (e != cudaSuccess) { set_error("conv_ws smem attribute: %s", cudaGetErrorString(e)); return DVMVS_ELAUNCH; }
+  }
+  p.w_bytes = kWsRows * kc_max * 2;
+  p.a_bytes = NPIX * kc_max * 2;
+  p.stage_bytes = (p.terms > 1 ? 2 : 1) * (p.a_bytes + p.w_bytes);
+  // the ring is sized for the weight stream: up to kWsRingBytes in flight (64-80 KiB of weights per CTA at 1 term), never more
+  // stages than the CTA has K chunks
+  int chunks_per_tap = 0;
+  for (int i = 0; i < p.n_src; ++i) chunks_per_tap += p.src_chunks[i];
+  const int cta_chunks = ((p.ksize * p.ksize + p.ksplit - 1) / p.ksplit) * chunks_per_tap;
+  const int stages = max(2, min(min(kMaxStages, cta_chunks), kWsRingBytes / p.stage_bytes));
+  p.num_stages = stages;
+  p.ring_bytes = max(stages * p.stage_bytes, NPIX * (kWsRows + 4) * 4);
+  const int smem = p.ring_bytes + 1024 + kBarrierBytes;
+  launch_k(conv_ws_kernel<NPIX>, grid, dim3(kTcThreads), (size_t)smem, s, p);
+  return check_launch("conv_ws_kernel");
+}
+
+// How dvmvs_conv2d_tc runs a descriptor: output tile, split count, and which kernel.  One function for the launch and for
+// dvmvs_conv2d_tc_ksplit, so the split count a deferred caller reads is the one the launch uses.
+struct TcPlan {
+  int Hout, Wout, tile_w, tile_h, tiles_x, tiles_y, ksplit;
+  bool ws;           // conv_ws_kernel (weights on the MMA's M side) instead of conv_tc_kernel
+};
+
+static TcPlan tc_plan(const dvmvs_conv_tc_desc* d) {
+  TcPlan t;
+  const int pad = (d->ksize - 1) / 2;
+  t.Hout = (d->Hin + 2 * pad - d->ksize) / d->stride + 1;
+  t.Wout = (d->Win + 2 * pad - d->ksize) / d->stride + 1;
+  // output-pixel tile: 16 wide x 8 high, or 8 x 16 for narrow maps
+  t.tile_w = (t.Wout <= 8 && t.Hout > 8) ? 8 : 16;
+  t.tile_h = kTileM / t.tile_w;
+  t.tiles_x = (t.Wout + t.tile_w - 1) / t.tile_w;
+  t.tiles_y = (t.Hout + t.tile_h - 1) / t.tile_h;
+  t.ksplit = 1;
+  t.ws = false;
+  const int n_tiles = (d->Cout + d->block_n - 1) / d->block_n;
+  const int ctas = t.tiles_x * t.tiles_y * d->B * n_tiles;
+  const int n_taps = d->ksize * d->ksize;
+  const size_t out_elems = (size_t)d->B * t.Hout * t.Wout * d->Cout;
+  const int n_sms = device_sm_count();
+  if (!(d->allow_split && d->workspace && d->workspace_bytes > kWsCounterBytes && ctas < n_sms / 2 && n_taps > 1)) return t;
+  const long long fit = (d->workspace_bytes - kWsCounterBytes) / (long long)(out_elems * sizeof(float));
+  // Weight-streaming kernel: a subset of the launches that split anyway (the same layers split, the partial sums keep their
+  // layout).  Stride 1 or 2 (the activation box strides like conv_tc_kernel's), no residual / aux (the finishing pass would
+  // apply them, but no such layer is weight-bound), fp16
+  // operand rows in whole 128-row blocks, Cout % 8 == 0 (16-byte partial-sum stores), at most kWsMaxPixels output pixels per
+  // image.  The split count aims for about kWsTargetCtas CTAs: fewer, longer weight streams than conv_tc_kernel's one CTA per
+  // SM per split, leaving SMs to the kernels of the other streams.
+  if (d->residual_mode == DVMVS_RES_NONE && !d->aux_out && d->Cout % 8 == 0 && d->w_rows % kWsRows == 0 &&
+      t.Hout * t.Wout <= kWsMaxPixels) {
+    int tw = t.tile_w, th = t.tile_h;
+    if (t.Hout <= 8 && t.Wout <= 8) tw = th = 8;
+    const int tx = (t.Wout + tw - 1) / tw, ty = (t.Hout + th - 1) / th;
+    const int base_ctas = tx * ty * d->B * ((d->Cout + kWsRows - 1) / kWsRows);
+    int k = (int)min((long long)min(n_taps, max(2, (kWsTargetCtas + base_ctas - 1) / base_ctas)), fit);
+    if (k >= 2) {
+      const int per = (n_taps + k - 1) / k;
+      t.ksplit = (n_taps + per - 1) / per;
+      t.ws = true;
+      t.tile_w = tw; t.tile_h = th; t.tiles_x = tx; t.tiles_y = ty;
+      return t;
+    }
+  }
+  t.ksplit = (int)max(1LL, min((long long)min(n_taps, (n_sms + ctas - 1) / ctas), fit));
+  const int per = (n_taps + t.ksplit - 1) / t.ksplit;
+  t.ksplit = (n_taps + per - 1) / per;              // no empty splits
+  return t;
+}
+
 }  // namespace dvmvs
 
 using namespace dvmvs;
@@ -587,16 +846,12 @@ extern "C" int dvmvs_conv2d_tc(const dvmvs_conv_tc_desc* d, dvmvs_stream_t strea
   DVMVS_REQUIRE(d->out_planes == nullptr || d->Cout % 8 == 0, "conv2d_tc: fp16-pair output needs Cout %% 8 == 0");
   TcParams p;
   memset(&p, 0, sizeof(p));
-  const int pad = (d->ksize - 1) / 2;
-  p.ksize = d->ksize; p.pad = pad; p.stride = d->stride;
-  p.Hout = (d->Hin + 2 * pad - d->ksize) / d->stride + 1;
-  p.Wout = (d->Win + 2 * pad - d->ksize) / d->stride + 1;
+  const TcPlan plan = tc_plan(d);
+  p.ksize = d->ksize; p.pad = (d->ksize - 1) / 2; p.stride = d->stride;
+  p.Hout = plan.Hout; p.Wout = plan.Wout;
   p.B = d->B; p.Cout = d->Cout;
-  // output-pixel tile: 16 wide x 8 high, or 8 x 16 for narrow maps
-  p.tile_w = (p.Wout <= 8 && p.Hout > 8) ? 8 : 16;
-  p.tile_h = kTileM / p.tile_w;
-  p.tiles_x = (p.Wout + p.tile_w - 1) / p.tile_w;
-  p.tiles_y = (p.Hout + p.tile_h - 1) / p.tile_h;
+  p.tile_w = plan.tile_w; p.tile_h = plan.tile_h;
+  p.tiles_x = plan.tiles_x; p.tiles_y = plan.tiles_y;
   p.n_src = d->n_src; p.terms = d->terms;
   int k_per_tap = 0, kc_max = 32;
   for (int s = 0; s < d->n_src; ++s) {
@@ -619,12 +874,13 @@ extern "C" int dvmvs_conv2d_tc(const dvmvs_conv_tc_desc* d, dvmvs_stream_t strea
   p.k_per_tap = k_per_tap;
   DVMVS_REQUIRE(d->ktot == k_per_tap * d->ksize * d->ksize, "conv2d_tc: packed weight K=%d, expected %d", d->ktot,
                 k_per_tap * d->ksize * d->ksize);
+  const int w_box_rows = plan.ws ? kWsRows : d->block_n;
   for (int kind = 0; kind < 2; ++kind) {
     const int kc = kind ? 64 : 32;
-    int rc = make_w_map(&p.w_map[kind][0], d->w_hi, d->w_rows, d->ktot, kc, d->block_n);
+    int rc = make_w_map(&p.w_map[kind][0], d->w_hi, d->w_rows, d->ktot, kc, w_box_rows);
     if (rc != DVMVS_OK) return rc;
     if (d->terms > 1) {
-      rc = make_w_map(&p.w_map[kind][1], d->w_lo, d->w_rows, d->ktot, kc, d->block_n);
+      rc = make_w_map(&p.w_map[kind][1], d->w_lo, d->w_rows, d->ktot, kc, w_box_rows);
       if (rc != DVMVS_OK) return rc;
     }
   }
@@ -642,29 +898,26 @@ extern "C" int dvmvs_conv2d_tc(const dvmvs_conv_tc_desc* d, dvmvs_stream_t strea
   p.hi_only = d->out_hi_only ? 1 : 0;
   cudaStream_t s = (cudaStream_t)stream;
   const int n_tiles = (d->Cout + d->block_n - 1) / d->block_n;
-  const int ctas = p.tiles_x * p.tiles_y * d->B * n_tiles;
-  p.ksplit = 1;
-  const int n_taps = d->ksize * d->ksize;
+  p.ksplit = plan.ksplit;
   // the first 16 KiB of the workspace are reserved (historical: arrival counters); the partial sums follow
-  const long long counter_bytes = 16384;
-  p.workspace = d->workspace ? reinterpret_cast<float*>(reinterpret_cast<char*>(d->workspace) + counter_bytes) : nullptr;
+  p.workspace = d->workspace ? reinterpret_cast<float*>(reinterpret_cast<char*>(d->workspace) + kWsCounterBytes) : nullptr;
   const size_t out_elems = (size_t)d->B * p.Hout * p.Wout * d->Cout;
-  const int n_sms = device_sm_count();
-  if (d->allow_split && d->workspace && d->workspace_bytes > counter_bytes && ctas < n_sms / 2 && n_taps > 1) {
-    long long fit = (d->workspace_bytes - counter_bytes) / (long long)(out_elems * sizeof(float));
-    p.ksplit = (int)max(1LL, min((long long)min(n_taps, (n_sms + ctas - 1) / ctas), fit));
-    const int per = (n_taps + p.ksplit - 1) / p.ksplit;
-    p.ksplit = (n_taps + per - 1) / per;              // no empty splits
-  }
-  dim3 grid(p.tiles_x * p.tiles_y * d->B, n_tiles, p.ksplit);
   // Measured and removed on the previous architecture: reducing the splits inside a thread-block cluster through distributed
   // shared memory (clusters of 5 / 9 one-CTA-per-SM blocks schedule worse than the short finishing launches they save) and a
   // fused finish by the last-arriving CTA (one CTA walks ksplit x BLOCK_N/8 dependent L2 round trips where the finishing
   // kernel spreads them over the GPU under the next prologue).
   int rc;
-  if (d->block_n == 32) rc = launch_tc<32>(p, grid, kc_max, s);
-  else if (d->block_n == 64) rc = launch_tc<64>(p, grid, kc_max, s);
-  else rc = launch_tc<128>(p, grid, kc_max, s);
+  if (plan.ws) {
+    const dim3 grid(p.tiles_x * p.tiles_y * d->B, (d->Cout + kWsRows - 1) / kWsRows, p.ksplit);
+    if (p.tile_w * p.tile_h == 64) rc = launch_ws<64>(p, grid, kc_max, s);
+    else rc = launch_ws<128>(p, grid, kc_max, s);
+  } else if (d->block_n == 32) {
+    rc = launch_tc<32>(p, dim3(p.tiles_x * p.tiles_y * d->B, n_tiles, p.ksplit), kc_max, s);
+  } else if (d->block_n == 64) {
+    rc = launch_tc<64>(p, dim3(p.tiles_x * p.tiles_y * d->B, n_tiles, p.ksplit), kc_max, s);
+  } else {
+    rc = launch_tc<128>(p, dim3(p.tiles_x * p.tiles_y * d->B, n_tiles, p.ksplit), kc_max, s);
+  }
   if (rc != DVMVS_OK) return rc;
   if (d->defer_finish) {
     // the caller's own epilogue kernel sums the split-K partial sums (dvmvs_lstm_gates_parts): only legal when this launch split
@@ -679,27 +932,10 @@ extern "C" int dvmvs_conv2d_tc(const dvmvs_conv_tc_desc* d, dvmvs_stream_t strea
 }
 
 // Split count dvmvs_conv2d_tc will use for this descriptor (1 = no split): lets a caller that fuses the finishing pass into its own
-// epilogue (defer_finish) size its reads.  Mirrors the decision above.
+// epilogue (defer_finish) size its reads.  The same plan as the launch (tc_plan).
 extern "C" int dvmvs_conv2d_tc_ksplit(const dvmvs_conv_tc_desc* d) {
   if (!d || !(d->ksize == 1 || d->ksize == 3 || d->ksize == 5) || d->B <= 0) return 1;
-  const int pad = (d->ksize - 1) / 2;
-  const int Hout = (d->Hin + 2 * pad - d->ksize) / d->stride + 1, Wout = (d->Win + 2 * pad - d->ksize) / d->stride + 1;
-  const int tile_w = (Wout <= 8 && Hout > 8) ? 8 : 16, tile_h = kTileM / tile_w;
-  const int tiles = ((Wout + tile_w - 1) / tile_w) * ((Hout + tile_h - 1) / tile_h);
-  const int n_tiles = (d->Cout + d->block_n - 1) / d->block_n;
-  const int ctas = tiles * d->B * n_tiles;
-  const int n_taps = d->ksize * d->ksize;
-  const long long counter_bytes = 16384;
-  const size_t out_elems = (size_t)d->B * Hout * Wout * d->Cout;
-  int ksplit = 1;
-  const int n_sms = device_sm_count();
-  if (d->allow_split && d->workspace && d->workspace_bytes > counter_bytes && ctas < n_sms / 2 && n_taps > 1) {
-    long long fit = (d->workspace_bytes - counter_bytes) / (long long)(out_elems * sizeof(float));
-    ksplit = (int)max(1LL, min((long long)min(n_taps, (n_sms + ctas - 1) / ctas), fit));
-    const int per = (n_taps + ksplit - 1) / ksplit;
-    ksplit = (n_taps + per - 1) / per;
-  }
-  return ksplit;
+  return tc_plan(d).ksplit;
 }
 
 extern "C" int dvmvs_split_planes(const float* x, void* planes, int B, int H, int W, int C, int Cs, int upsample2x, int c_offset,
